@@ -38,7 +38,7 @@ extern "C" {
 #endif
 
 #define OLB_VERSION_MAJOR 0
-#define OLB_VERSION_MINOR 1
+#define OLB_VERSION_MINOR 2
 
 /* ---- error codes ------------------------------------------------------- */
 #define OLB_OK                 0
@@ -105,12 +105,12 @@ extern "C" {
 #define OLB_AP_INTERSECT   17  /* pops 2, pushes a & b                                */
 #define OLB_AP_DIFFERENCE  18  /* pops 2, pushes a & ~b                               */
 
-/* ---- trace flags (argument `flags` of olb_trace_*) ------------------------ */
+/* ---- trace flags (OlbTraceCall.flags, `flags` of olb_trace_host_*) -------- */
 #define OLB_TF_POLARIZED   (1u << 0)  /* rays carry a 3x3 complex P matrix (OlbRays.p)  */
 #define OLB_TF_POL_IDENTITY (1u << 2) /* with POLARIZED: P starts as identity, rays.p is output only */
 #define OLB_TF_SHARED_INPUT (1u << 4) /* batched trace: every system traces the SAME rays_per_system launch rays */
 #define OLB_TF_MOMENTS     (1u << 3)  /* accumulate OlbMoments over the traced batch (fused analysis
-                                         epilogue, SURVEY.md 8f-2); see olb_trace_moments_*          */
+                                         epilogue, SURVEY.md 8f-2); see OlbTraceCall.moments         */
 #define OLB_TF_MOMENTS_GLOBAL (1u << 5) /* moments of the GLOBAL (x, y) of the last traced surface instead of its local frame */
 #define OLB_TF_MOMENTS_ALL (1u << 6)  /* moments over EVERY ray (no i > 0 / finite mask): a NaN ray makes the sums NaN, like
                                          be.mean over the record row in the rms_spot_size operand (operand/ray.py:337-341) */
@@ -183,7 +183,7 @@ typedef struct OlbSurface {
  */
 
 /* The whole table: surfaces + pool + wavelength list. Host or device memory
- * (host for olb_trace_*: the library stages it; it is < 64 KiB). */
+ * (host for olb_table_upload: the library stages it; it is < 64 KiB). */
 typedef struct OlbTable {
   const OlbSurface* surfaces;  /* n_surfaces entries                           */
   int32_t n_surfaces;
@@ -247,7 +247,7 @@ int olb_last_error(char* buf, int buf_len);
 
 /*
  * Device-resident ("prepared") table handle.  Filled by olb_table_upload; a plain
- * caller-owned struct (the library keeps no registry): pass it to olb_trace_*.
+ * caller-owned struct (the library keeps no registry): pass it to the trace entry points.
  * `workspace` is caller-allocated DEVICE memory of >= olb_table_workspace_bytes().
  */
 typedef struct OlbDeviceTable {
@@ -260,7 +260,7 @@ typedef struct OlbDeviceTable {
   int32_t off_f64, bytes_f64;   /* fp64 blob inside workspace */
   int32_t off_f32, bytes_f32;   /* fp32 blob inside workspace */
   int32_t bwd_supported;        /* 1 if olb_trace_bwd_* covers every surface of the table; 2: covered, and the table has
-                                   polynomial / Zernike / Chebyshev / Forbes surfaces, which need olb_trace_bwd_tables_* */
+                                   polynomial / Zernike / Chebyshev / Forbes surfaces, which need grad_tables */
   int32_t bwd_slots;            /* gradient accumulator slots per thread (backward kernel)   */
   int32_t n_systems;            /* 1, or the number of systems of a batched table            */
   int32_t stride_f64;           /* bytes between consecutive systems' fp64 / fp32 blobs      */
@@ -283,23 +283,6 @@ int64_t olb_table_workspace_bytes(const OlbTable* table);
  */
 int olb_table_upload(const OlbTable* table, void* workspace, int64_t workspace_bytes,
                      void* stream, OlbDeviceTable* out);
-
-/*
- * Trace n_rays rays through surfaces [first, last) of the prepared table.
- * Replaces SurfaceGroup.trace(rays, skip=first) (surface_group.py:245-257) --
- * and, with last = first + 1, a single Surface.trace as issued by the ray
- * aimers (optiland/rays/ray_aiming/iterative.py:366).
- *   rays      : device SoA (updated in place unless OLB_TF_NO_FINAL)
- *   rec       : optional record rows, row r <-> surface first + r
- *   status    : optional device int32, OR-ed with OLB_ST_* bits
- * Asynchronous on `stream`.
- */
-int olb_trace_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                  const OlbRays* rays, const OlbRecords* rec, int64_t n_rays,
-                  uint32_t flags, int32_t* status, void* stream);
-int olb_trace_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                  const OlbRays* rays, const OlbRecords* rec, int64_t n_rays,
-                  uint32_t flags, int32_t* status, void* stream);
 
 /*
  * Launch state from pupil coordinates (the step immediately before the path, SURVEY.md 8f-1):
@@ -348,73 +331,29 @@ typedef struct OlbPupilLaunch {
 #define OLB_MAX_VIG_FIELDS 16
 
 /*
- * As olb_trace_*, but the launch state comes from `launch`.  `out` receives the final state
- * (x,y,z,L,M,N,i,opd; not needed with OLB_TF_NO_FINAL) and supplies `w` when the table has several
- * wavelengths.  Record row 0 of an object surface holds the generated launch state.
- */
-int olb_trace_pupil_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                        const OlbPupilLaunch* launch, const OlbRays* out, const OlbRecords* rec,
-                        int64_t n_rays, uint32_t flags, int32_t* status, void* stream);
-int olb_trace_pupil_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                        const OlbPupilLaunch* launch, const OlbRays* out, const OlbRecords* rec,
-                        int64_t n_rays, uint32_t flags, int32_t* status, void* stream);
-
-/*
- * Fused analysis epilogue (the step immediately after the path): moments of the ray intercepts on the
- * LAST traced surface, in that surface's local frame (what SpotDiagram transforms to,
- * optiland/analysis/spot_diagram/core.py:462-481), over rays with intensity > 0 and finite intercepts
- * (the mask of core.py:471-472), relative to `center`:
- *   m[0] = count, m[1] = sum (x - cx), m[2] = sum (y - cy), m[3] = sum ((x-cx)^2 + (y-cy)^2),
- *   m[4] = sum intensity, m[5] = sum opd, m[6] = sum opd^2,
- *   m[7] = number of rays with intensity > 0 whose intercept is NOT finite (the reference's mask keeps them, so its
- *          statistics are NaN whenever this is non-zero)
- * accumulated in fp64 INTO `moments` (device, 8 doubles; the caller zeroes it).  From these follow the
- * centroid, the RMS spot radius about the centroid or about `center` (rms_spot_radius, core.py:357-370)
- * and the OPD mean / variance without writing or re-reading any per-ray array: rec may be NULL and
- * with OLB_TF_NO_FINAL the trace writes nothing per ray.  `launch` (optional) as in olb_trace_pupil_*.
- */
-int olb_trace_moments_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                          const OlbPupilLaunch* launch, const OlbRays* rays, const OlbRecords* rec,
-                          int64_t n_rays, uint32_t flags, const double center[2], double* moments,
-                          int32_t* status, void* stream);
-int olb_trace_moments_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                          const OlbPupilLaunch* launch, const OlbRays* rays, const OlbRecords* rec,
-                          int64_t n_rays, uint32_t flags, const double center[2], double* moments,
-                          int32_t* status, void* stream);
-
-/*
  * Host-buffer end-to-end trace: HOST SoA in, HOST final ray state out, the
  * per-surface records stay on the device (rec, optional).  Rays are cut into
  * chunks; H2D copy, kernel and D2H copy of consecutive chunks overlap on three
  * streams.  `h_in` supplies x,y,z,L,M,N,i,w (opd ignored, starts at 0);
  * `h_out` receives x,y,z,L,M,N,i,opd.  Host buffers should be pinned.
  *   dev_scratch : device memory, >= olb_host_scratch_bytes(elem_size, chunk)
+ * With `launch` (optional) the launch state is generated on the device from HOST pupil arrays instead
+ * (launch->Px, launch->Py are host pointers; h_in may be NULL): 8 B/ray cross PCIe instead of 28-32 B/ray.
+ * launch->Hx / Hy (host arrays, optional, together) give every ray its own field point --
+ * RealRayTracer.trace_generic's call shape; for a table with several wavelengths the per-ray wavelengths are
+ * then read from h_out->w (host).
  */
 int64_t olb_host_scratch_bytes(int32_t elem_size, int64_t chunk_rays);
 int olb_trace_host_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                       const OlbRays* h_in, const OlbRays* h_out,
+                       const OlbPupilLaunch* launch, const OlbRays* h_in, const OlbRays* h_out,
                        const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
                        void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags,
                        int32_t* status);
 int olb_trace_host_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                       const OlbRays* h_in, const OlbRays* h_out,
+                       const OlbPupilLaunch* launch, const OlbRays* h_in, const OlbRays* h_out,
                        const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
                        void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags,
                        int32_t* status);
-/* Same pipeline with the launch state generated on the device from HOST pupil arrays
- * (launch->Px, launch->Py are host pointers): 8 B/ray cross PCIe instead of 28-32 B/ray.  launch->Hx / Hy (host
- * arrays, optional, together) give every ray its own field point -- RealRayTracer.trace_generic's call shape; for a
- * table with several wavelengths the per-ray wavelengths are read from h_out->w (host). */
-int olb_trace_host_pupil_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                             const OlbPupilLaunch* launch, const OlbRays* h_out,
-                             const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
-                             void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags,
-                             int32_t* status);
-int olb_trace_host_pupil_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                             const OlbPupilLaunch* launch, const OlbRays* h_out,
-                             const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
-                             void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags,
-                             int32_t* status);
 
 /*
  * Reverse mode (the backward pass of the autograd configuration; reference:
@@ -449,18 +388,11 @@ int olb_trace_host_pupil_f64(const OlbDeviceTable* table, int32_t first, int32_t
 #define OLB_GP_MAX_COEF 12
 #define OLB_GP_R (OLB_GP_COEF + OLB_GP_MAX_COEF)   /* 9 entries, row-major: dLoss/dR of a tilted pose */
 #define OLB_GP_COUNT (OLB_GP_R + 9)
-int olb_trace_bwd_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                      const OlbRays* rays_in, const OlbRecords* rec, const OlbRecords* grad_rec,
-                      const OlbRays* grad_rays_in, double* grad_params, int64_t n_rays,
-                      uint64_t grad_row_mask, void* stream);
-int olb_trace_bwd_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                      const OlbRays* rays_in, const OlbRecords* rec, const OlbRecords* grad_rec,
-                      const OlbRays* grad_rays_in, double* grad_params, int64_t n_rays,
-                      uint64_t grad_row_mask, void* stream);
 
 /*
- * The same with TABLE gradients for the polynomial families (OlbDeviceTable.bwd_supported == 2: the table holds
- * OLB_GEOM_POLYNOMIAL / OLB_GEOM_ZERNIKE / OLB_GEOM_CHEBYSHEV surfaces of at most 12 x 12 monomials).  The adjoint goes through the
+ * grad_tables: TABLE gradients for the polynomial families, required when OlbDeviceTable.bwd_supported == 2 (the
+ * table holds OLB_GEOM_POLYNOMIAL / OLB_GEOM_ZERNIKE / OLB_GEOM_CHEBYSHEV surfaces of at most 12 x 12 monomials) and
+ * ignored (may be NULL) when it is 1.  The adjoint goes through the
  * intersection by the implicit-function theorem with the TRUE gradient of the sag polynomial and through the normal with
  * the Hessian of the reference's slope polynomial (whose Zernike form omits the normalisation constants,
  * optiland/zernike/base.py:104-136).  grad_tables: n_surfaces blocks of OLB_GT_PER_SURFACE doubles, ACCUMULATED --
@@ -472,7 +404,7 @@ int olb_trace_bwd_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
  * Chebyshev: ONE table S = D = P with P_pq = sum_ij C_ij Tc[i][p] Tc[j][q] (Tc: monomial coefficients of T_n), its slope
  * entering the normal WITHOUT the factors 1 / norm_x, 1 / norm_y (the reference's form, chebyshev.py:171-181), so
  * dLoss/dC_ij = sum_pq Tc[i][p] (dLoss/dS + dLoss/dD)_pq Tc[j][q].
- * OLB_GEOM_FORBES_QBFS surfaces (at most 12 radial terms) are covered by this entry point as well (they use none of the
+ * OLB_GEOM_FORBES_QBFS surfaces (at most 12 radial terms) also make bwd_supported 2 (they use none of the
  * table blocks): grad_params[OLB_GP_COEF + m] receives dLoss/db_m, b = the coefficients of the basis the Clenshaw
  * recurrence runs on (A b = a with the upper-banded f / g / h matrix of Forbes, Opt. Express 18, 19700 (2010),
  * eqs. A.14-A.16; optiland/geometries/forbes/qpoly.py:56-115), so dLoss/da = A^-T dLoss/db
@@ -480,17 +412,18 @@ int olb_trace_bwd_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
  */
 #define OLB_GT_DIM 12
 #define OLB_GT_PER_SURFACE (2 * OLB_GT_DIM * OLB_GT_DIM)
-int olb_trace_bwd_tables_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                             const OlbRays* rays_in, const OlbRecords* rec, const OlbRecords* grad_rec,
-                             const OlbRays* grad_rays_in, double* grad_params, double* grad_tables, int64_t n_rays,
-                             uint64_t grad_row_mask, void* stream);
-int olb_trace_bwd_tables_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                             const OlbRays* rays_in, const OlbRecords* rec, const OlbRecords* grad_rec,
-                             const OlbRays* grad_rays_in, double* grad_params, double* grad_tables, int64_t n_rays,
-                             uint64_t grad_row_mask, void* stream);
+int olb_trace_bwd_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
+                      const OlbRays* rays_in, const OlbRecords* rec, const OlbRecords* grad_rec,
+                      const OlbRays* grad_rays_in, double* grad_params, double* grad_tables, int64_t n_rays,
+                      uint64_t grad_row_mask, void* stream);
+int olb_trace_bwd_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
+                      const OlbRays* rays_in, const OlbRecords* rec, const OlbRecords* grad_rec,
+                      const OlbRays* grad_rays_in, double* grad_params, double* grad_tables, int64_t n_rays,
+                      uint64_t grad_row_mask, void* stream);
 
 /*
- * Fused wavefront epilogue (SURVEY.md 8f-2, second half): instead of (or besides) records / the final state,
+ * Fused wavefront epilogue (SURVEY.md 8f-2, second half; OlbTraceCall.wavefront_ref / wavefront_out, optional,
+ * together): instead of (or besides) records / the final state,
  * the trace writes per ray the OPD in waves against a spherical reference and the point where the ray meets
  * that sphere -- steps 4-5 of ChiefRayStrategy.compute_wavefront_data
  * (optiland/wavefront/strategy.py:179-190) on top of SphericalReference.path_length
@@ -502,6 +435,7 @@ int olb_trace_bwd_tables_f64(const OlbDeviceTable* table, int32_t first, int32_t
  * infinite-object angle field, else 0 (it needs `launch`, the pupil samples).  The caller computes centre,
  * radius and opd_ref from the chief ray (one ordinary 1-ray trace).  Evaluated in fp64 for both element types.
  * `last` must be the image surface.  With OLB_TF_NO_FINAL and rec == NULL nothing else is written per ray.
+ * Not built for batched systems.
  */
 typedef struct {
   double center[3];
@@ -518,18 +452,10 @@ typedef struct {
   void* pupil_z;
   void* intensity;
 } OlbWavefrontOut;
-int olb_trace_wavefront_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                            const OlbPupilLaunch* launch, const OlbRays* rays, const OlbRecords* rec,
-                            int64_t n_rays, uint32_t flags, const OlbWavefrontRef* ref,
-                            const OlbWavefrontOut* out, int32_t* status, void* stream);
-int olb_trace_wavefront_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                            const OlbPupilLaunch* launch, const OlbRays* rays, const OlbRecords* rec,
-                            int64_t n_rays, uint32_t flags, const OlbWavefrontRef* ref,
-                            const OlbWavefrontOut* out, int32_t* status, void* stream);
 
 /*
- * Polarized call shapes (config 5): PolarizedRays through the fused launch / the wavefront epilogue, with the
- * intensity epilogue of RealRayTracer.trace in-kernel.
+ * Polarized call shapes (config 5, OLB_TF_POLARIZED): PolarizedRays through the fused launch / the wavefront
+ * epilogue, with the intensity epilogue of RealRayTracer.trace in-kernel (OlbTraceCall.pol).
  *
  * `pol` describes optic.polarization_state (optiland/rays/polarization_state.py:15-56) and asks for
  * PolarizedRays.update_intensity (optiland/rays/polarized_rays.py:122-133 with _get_3d_electric_field :204-233):
@@ -541,10 +467,9 @@ int olb_trace_wavefront_f64(const OlbDeviceTable* table, int32_t first, int32_t 
  * wavefront epilogue's out.intensity receives the updated value.  A launch direction parallel to xhat sets
  * OLB_ST_K_PARALLEL_X (the reference raises).
  *
- * OLB_TF_POLARIZED is implied.  `launch` (optional) as in olb_trace_pupil_*: P then starts as the identity
- * (PolarizedRays.__init__, :50) and rays.p is output only -- and may be NULL when pol is given (the P matrices are
- * then not written at all: 72 / 144 B per ray saved).  `ref` / `out` (optional, together) as in
- * olb_trace_wavefront_*.  pol may be NULL (plain polarized trace: P matrices only).
+ * `pol` needs OLB_TF_POLARIZED in flags.  With `launch`, P starts as the identity (PolarizedRays.__init__, :50) and
+ * rays.p is output only -- and may be NULL when pol is given (the P matrices are then not written at all: 72 / 144 B
+ * per ray saved).  pol may be NULL (plain polarized trace: P matrices only).
  */
 typedef struct OlbPolarization {
   int32_t is_polarized;     /* 0: unpolarized (mean of two orthogonal states); 1: (Ex, Ey, phase_x, phase_y) */
@@ -553,17 +478,9 @@ typedef struct OlbPolarization {
   double phase_x, phase_y;  /* radians                                                                      */
   void* intensity;          /* optional device output, n_rays elements of the kernel's type                 */
 } OlbPolarization;
-int olb_trace_polarized_f32(const OlbDeviceTable* table, int32_t first, int32_t last,
-                            const OlbPupilLaunch* launch, const OlbRays* rays, const OlbRecords* rec,
-                            int64_t n_rays, uint32_t flags, const OlbPolarization* pol,
-                            const OlbWavefrontRef* ref, const OlbWavefrontOut* out, int32_t* status, void* stream);
-int olb_trace_polarized_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
-                            const OlbPupilLaunch* launch, const OlbRays* rays, const OlbRecords* rec,
-                            int64_t n_rays, uint32_t flags, const OlbPolarization* pol,
-                            const OlbWavefrontRef* ref, const OlbWavefrontOut* out, int32_t* status, void* stream);
 
 /*
- * Batched many-systems trace (SURVEY.md 8f-4): B perturbed copies of one template system -- the shape of
+ * Batched many-systems tables (SURVEY.md 8f-4): B perturbed copies of one template system -- the shape of
  * tolerancing Monte-Carlo runs (optiland/tolerancing/monte_carlo.py) and of the BatchedRayEvaluator
  * (optiland/optimization/batched_evaluator.py:277-705), which the reference evaluates as B separate small
  * traces.  `params` (HOST): n_systems x n_surfaces blocks of OLB_BP_COUNT doubles with the ABSOLUTE values
@@ -571,10 +488,7 @@ int olb_trace_polarized_f64(const OlbDeviceTable* table, int32_t first, int32_t 
  *   coordinate_system.py:145-165, as in OlbSurface.t / .R), [OLB_BP_CURV] 1/radius, [OLB_BP_CONIC], [OLB_BP_N1], [OLB_BP_N2],
  *   [OLB_BP_COEF + j] even-asphere coefficients;
  * everything else (kinds, apertures, coatings, tolerances) comes from `template_table` (one wavelength).
- * olb_trace_batch_* traces system b over the ray segment [b * rays_per_system, (b+1) * rays_per_system): ONE
- * launch, grid.y = system, each CTA stages its own system's table.  With OLB_TF_SHARED_INPUT (+ NO_FINAL) all
- * systems read the same rays_per_system launch rays.  rec rows have n_systems * rays_per_system columns;
- * `moments` (optional) receives 8 doubles PER SYSTEM (see olb_trace_moments_*).
+ * Traced by olb_trace_call_* with OlbTraceCall.rays_per_system.
  */
 #define OLB_BP_TX 0
 #define OLB_BP_TY 1
@@ -590,12 +504,53 @@ int olb_trace_polarized_f64(const OlbDeviceTable* table, int32_t first, int32_t 
 int64_t olb_table_batch_workspace_bytes(const OlbTable* template_table, int32_t n_systems);
 int olb_table_upload_batch(const OlbTable* template_table, const double* params, int32_t n_systems,
                            void* workspace, int64_t workspace_bytes, void* stream, OlbDeviceTable* out);
-int olb_trace_batch_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays,
-                        const OlbRecords* rec, int64_t rays_per_system, uint32_t flags,
-                        const double center[2], double* moments, int32_t* status, void* stream);
-int olb_trace_batch_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays,
-                        const OlbRecords* rec, int64_t rays_per_system, uint32_t flags,
-                        const double center[2], double* moments, int32_t* status, void* stream);
+
+/*
+ * Forward trace on device buffers: n_rays rays through surfaces [first, last) of the prepared table.
+ * Replaces SurfaceGroup.trace(rays, skip=first) (surface_group.py:245-257) -- and, with last = first + 1, a single
+ * Surface.trace as issued by the ray aimers (optiland/rays/ray_aiming/iterative.py:366).  Every optional stage
+ * is switched on by its field of OlbTraceCall; every pointer may be NULL.  Asynchronous on `stream`.
+ */
+typedef struct OlbTraceCall {
+  int32_t first, last;
+  int64_t n_rays;
+  uint32_t flags;             /* OLB_TF_*                                                                        */
+  int32_t reserved;
+  /* Device SoA (updated in place unless OLB_TF_NO_FINAL).  With `launch` it receives the final state
+   * (x,y,z,L,M,N,i,opd; not needed with OLB_TF_NO_FINAL) and supplies `w` when the table has several wavelengths;
+   * then, and whenever nothing would be read or written, it may be NULL. */
+  const OlbRays* rays;
+  const OlbRecords* rec;      /* optional record rows, row r <-> surface first + r                              */
+  /* Launch state generated in-kernel from pupil coordinates (see OlbPupilLaunch) instead of read from rays.
+   * Record row 0 of an object surface holds the generated launch state. */
+  const OlbPupilLaunch* launch;
+  /* Fused analysis epilogue (the step immediately after the path): moments of the ray intercepts on the
+   * LAST traced surface, in that surface's local frame (what SpotDiagram transforms to,
+   * optiland/analysis/spot_diagram/core.py:462-481), over rays with intensity > 0 and finite intercepts
+   * (the mask of core.py:471-472), relative to `center`:
+   *   m[0] = count, m[1] = sum (x - cx), m[2] = sum (y - cy), m[3] = sum ((x-cx)^2 + (y-cy)^2),
+   *   m[4] = sum intensity, m[5] = sum opd, m[6] = sum opd^2,
+   *   m[7] = number of rays with intensity > 0 whose intercept is NOT finite (the reference's mask keeps them, so its
+   *          statistics are NaN whenever this is non-zero)
+   * accumulated in fp64 INTO `moments` (device, 8 doubles; the caller zeroes it).  From these follow the
+   * centroid, the RMS spot radius about the centroid or about `center` (rms_spot_radius, core.py:357-370)
+   * and the OPD mean / variance without writing or re-reading any per-ray array: rec may be NULL and
+   * with OLB_TF_NO_FINAL the trace writes nothing per ray.  moments != NULL implies OLB_TF_MOMENTS. */
+  double center[2];
+  double* moments;
+  /* Batched table (olb_table_upload_batch; required, > 0, when the table holds several systems): system b
+   * traces the ray segment [b * rays_per_system, (b+1) * rays_per_system), n_rays = n_systems * rays_per_system.
+   * ONE launch, grid.y = system, each CTA stages its own system's table.  With OLB_TF_SHARED_INPUT (+ NO_FINAL)
+   * all systems read the same rays_per_system launch rays.  rec rows have n_rays columns; `moments` receives
+   * 8 doubles PER SYSTEM.  0: a single-system table. */
+  int64_t rays_per_system;
+  const OlbWavefrontRef* wavefront_ref;   /* wavefront epilogue (above), together with wavefront_out            */
+  const OlbWavefrontOut* wavefront_out;
+  const OlbPolarization* pol;             /* polarized intensity epilogue (above)                               */
+  int32_t* status;            /* optional device int32, OR-ed with OLB_ST_* bits                                */
+} OlbTraceCall;               /* 112 bytes                                                                      */
+int olb_trace_call_f32(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream);
+int olb_trace_call_f64(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream);
 
 /*
  * Huygens-Fresnel PSF summation (SURVEY.md 8f-3; reference: NumbaSummation._huygens_fresnel_summation,

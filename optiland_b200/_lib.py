@@ -14,7 +14,7 @@ import numpy as np
 from . import table as T
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("OLB_LIB", os.path.join(_HERE, "libolb.so"))  # OLB_LIB: tuning builds only
+LIB_PATH = os.path.join(_HERE, "libolb.so")
 
 OK = 0
 ERRORS = {-1: "OLB_ERR_INVALID_ARG", -2: "OLB_ERR_UNSUPPORTED", -3: "OLB_ERR_CUDA",
@@ -76,6 +76,15 @@ class OlbPolarization(C.Structure):
                 ("phase_x", C.c_double), ("phase_y", C.c_double), ("intensity", C.c_void_p)]
 
 
+class OlbTraceCall(C.Structure):
+    _fields_ = [("first", C.c_int32), ("last", C.c_int32), ("n_rays", C.c_int64), ("flags", C.c_uint32),
+                ("reserved", C.c_int32), ("rays", C.POINTER(OlbRays)), ("rec", C.POINTER(OlbRecords)),
+                ("launch", C.POINTER(OlbPupilLaunch)), ("center", C.c_double * 2), ("moments", C.c_void_p),
+                ("rays_per_system", C.c_int64), ("wavefront_ref", C.POINTER(OlbWavefrontRef)),
+                ("wavefront_out", C.POINTER(OlbWavefrontOut)), ("pol", C.POINTER(OlbPolarization)),
+                ("status", C.c_void_p)]
+
+
 class OlbDeviceTable(C.Structure):
     _fields_ = [
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64), ("magic", C.c_uint32),
@@ -94,55 +103,17 @@ SYMBOLS = {
     "olb_launch_count": (C.c_int64, []),
     "olb_table_workspace_bytes": (C.c_int64, [_P(OlbTable)]),
     "olb_table_upload": (C.c_int, [_P(OlbTable), C.c_void_p, C.c_int64, C.c_void_p, _P(OlbDeviceTable)]),
-    "olb_trace_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
-                                C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p]),
-    "olb_trace_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
-                                C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "olb_trace_call_f32": (C.c_int, [_P(OlbDeviceTable), _P(OlbTraceCall), C.c_void_p]),
+    "olb_trace_call_f64": (C.c_int, [_P(OlbDeviceTable), _P(OlbTraceCall), C.c_void_p]),
     "olb_trace_bwd_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
-                                    _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p]),
+                                    _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64,
+                                    C.c_void_p]),
     "olb_trace_bwd_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
-                                    _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_int64, C.c_uint64, C.c_void_p]),
-    "olb_trace_bwd_tables_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
-                                           _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64,
-                                           C.c_void_p]),
-    "olb_trace_bwd_tables_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
-                                           _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64,
-                                           C.c_void_p]),
-    "olb_trace_pupil_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                      _P(OlbRecords), C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p]),
-    "olb_trace_pupil_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                      _P(OlbRecords), C.c_int64, C.c_uint32, C.c_void_p, C.c_void_p]),
-    "olb_trace_moments_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                        _P(OlbRecords), C.c_int64, C.c_uint32, _P(C.c_double), C.c_void_p,
-                                        C.c_void_p, C.c_void_p]),
-    "olb_trace_moments_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                        _P(OlbRecords), C.c_int64, C.c_uint32, _P(C.c_double), C.c_void_p,
-                                        C.c_void_p, C.c_void_p]),
-    "olb_trace_host_pupil_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                           _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
-                                           C.c_uint32, C.c_void_p]),
-    "olb_trace_host_pupil_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                           _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
-                                           C.c_uint32, C.c_void_p]),
-    "olb_trace_wavefront_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                          _P(OlbRecords), C.c_int64, C.c_uint32, _P(OlbWavefrontRef), _P(OlbWavefrontOut),
-                                          C.c_void_p, C.c_void_p]),
-    "olb_trace_wavefront_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                          _P(OlbRecords), C.c_int64, C.c_uint32, _P(OlbWavefrontRef), _P(OlbWavefrontOut),
-                                          C.c_void_p, C.c_void_p]),
-    "olb_trace_polarized_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                          _P(OlbRecords), C.c_int64, C.c_uint32, _P(OlbPolarization), _P(OlbWavefrontRef),
-                                          _P(OlbWavefrontOut), C.c_void_p, C.c_void_p]),
-    "olb_trace_polarized_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
-                                          _P(OlbRecords), C.c_int64, C.c_uint32, _P(OlbPolarization), _P(OlbWavefrontRef),
-                                          _P(OlbWavefrontOut), C.c_void_p, C.c_void_p]),
+                                    _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64,
+                                    C.c_void_p]),
     "olb_table_batch_workspace_bytes": (C.c_int64, [_P(OlbTable), C.c_int32]),
     "olb_table_upload_batch": (C.c_int, [_P(OlbTable), C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
                                          _P(OlbDeviceTable)]),
-    "olb_trace_batch_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords), C.c_int64,
-                                      C.c_uint32, _P(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p]),
-    "olb_trace_batch_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords), C.c_int64,
-                                      C.c_uint32, _P(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p]),
     "olb_huygens_psf_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_double,
                                       C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -151,11 +122,11 @@ SYMBOLS = {
     "olb_fft_psf_accumulate_f64": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
     "olb_fft_psf_accumulate_f32": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
     "olb_host_scratch_bytes": (C.c_int64, [C.c_int32, C.c_int64]),
-    "olb_trace_host_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRays),
-                                     _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
+    "olb_trace_host_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
+                                     _P(OlbRays), _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
                                      C.c_uint32, C.c_void_p]),
-    "olb_trace_host_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRays),
-                                     _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
+    "olb_trace_host_f64": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
+                                     _P(OlbRays), _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
                                      C.c_uint32, C.c_void_p]),
 }
 

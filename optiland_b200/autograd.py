@@ -1,4 +1,4 @@
-"""Differentiable trace: ``torch.autograd.Function`` over olb_trace_* / olb_trace_bwd_*.
+"""Differentiable trace: ``torch.autograd.Function`` over olb_trace_call_* / olb_trace_bwd_*.
 
 The reference obtains gradients by ``loss.backward()`` through the eager graph of every
 element-wise op of the trace (optiland/optimization/optimizer/torch/base.py:96-156),
@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from . import table as T
-from .trace import _DTYPES, _REC_KEYS, DeviceTable
+from .trace import _DTYPES, _REC_KEYS, DeviceTable, _c_records, _out_buffer, _trace
 
 GP_TX, GP_TY, GP_TZ, GP_CURV, GP_CONIC, GP_N1, GP_N2, GP_COEF = 0, 1, 2, 3, 4, 5, 6, 7
 GP_MAX_COEF = _lib.GP_MAX_COEF
@@ -156,7 +156,7 @@ def _coef_maps(table: T.SurfaceTable):
 
 
 def tables_to_coef_grads(table: T.SurfaceTable, gtab: np.ndarray, K: int) -> np.ndarray:
-    """(S, 2, 12, 12) table gradients of olb_trace_bwd_tables_* -> (S, K) gradients of the user coefficients."""
+    """(S, 2, 12, 12) table gradients of olb_trace_bwd_* (grad_tables) -> (S, K) gradients of the user coefficients."""
     out = np.zeros((table.num_surfaces, K))
     for s, m in _coef_maps(table).items():
         if m[0] == "zernike":
@@ -286,7 +286,6 @@ class _TraceFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, template, device_tables, rows, params, coefs, x, y, z, L, M, N, i, opd):
         ctx.set_materialize_grads(False)
-        lib = _lib.load()
         dtype = x.dtype
         sfx = _DTYPES[dtype]
         if device_tables and isinstance(device_tables[0], DeviceTable):
@@ -311,17 +310,11 @@ class _TraceFn(torch.autograd.Function):
         # (a slice / view of a larger tensor may start anywhere: the C ABI wants 16-byte aligned arrays)
         ins = [t.detach().contiguous() for t in (x, y, z, L, M, N, i, opd)]
         ins = [t.clone() if t.data_ptr() % 16 else t for t in ins]
-        vec = 4 if dtype == torch.float32 else 2
-        stride = n if n % vec == 0 else (n + 63) // 64 * 64
-        buf = torch.empty((8, S, stride), dtype=dtype, device=x.device)
-        c_rec = _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], stride)
+        buf = _out_buffer(8, S, n, dtype, x.device)
         c_rays = _lib.OlbRays(**{k: t.data_ptr() for k, t in zip(("x", "y", "z", "L", "M", "N", "i", "opd"), ins)})
-        with torch.cuda.device(x.device):
-            stream = torch.cuda.current_stream(x.device).cuda_stream
-            rc = getattr(lib, f"olb_trace_{sfx}")(C.byref(dtab.c), 0, S, C.byref(c_rays), C.byref(c_rec), n,
-                                                  _lib.TF_NO_FINAL, None, C.c_void_p(stream))
-        _lib.check(rc, f"olb_trace_{sfx}")
-        ctx.dtab, ctx.ins, ctx.buf, ctx.stride, ctx.sfx = dtab, ins, buf, stride, sfx
+        # (no status word: out-of-range freeform coordinates are not reported on this path)
+        _trace(dtab, x.device, dtype, 0, S, n, _lib.TF_NO_FINAL, rays=c_rays, rec=_c_records(buf), own_status=False)
+        ctx.dtab, ctx.ins, ctx.buf, ctx.sfx = dtab, ins, buf, sfx
         ctx.rows = None if rows is None else tuple(r % S for r in rows)
         ctx.params_on_device = params.is_cuda
         ctx.coefs_meta = None if coefs is None else (coefs.shape[1], coefs.is_cuda, coefs.dtype)
@@ -333,7 +326,7 @@ class _TraceFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         lib = _lib.load()
-        dtab, ins, buf, stride = ctx.dtab, ctx.ins, ctx.buf, ctx.stride
+        dtab, ins, buf = ctx.dtab, ctx.ins, ctx.buf
         n = ins[0].numel()
         S = buf.shape[1]
         dtype = buf.dtype
@@ -364,7 +357,7 @@ class _TraceFn(torch.autograd.Function):
                         gb[r].copy_(g)
                 gbufs.append(gb)
         c_grec = _lib.OlbRecords(*[(g.data_ptr() if g is not None else None) for g in gbufs], n)
-        c_rec = _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], stride)
+        c_rec = _c_records(buf)
         c_in = _lib.OlbRays(**{k: t.data_ptr() for k, t in zip(("x", "y", "z", "L", "M", "N", "i", "opd"), ins)})
         gin = [torch.empty_like(ins[0]) for _ in range(8)] if ctx.needs_ray_grad else None
         c_gin = _lib.OlbRays(**{k: t.data_ptr() for k, t in zip(("x", "y", "z", "L", "M", "N", "i", "opd"), gin)}) if gin else None
@@ -373,17 +366,12 @@ class _TraceFn(torch.autograd.Function):
         gtab = torch.zeros((S, 2, _lib.GT_DIM, _lib.GT_DIM), dtype=torch.float64, device=buf.device) if tables else None
         with torch.cuda.device(buf.device):
             stream = torch.cuda.current_stream(buf.device).cuda_stream
-            if tables:
-                # polynomial / Zernike / Chebyshev surfaces: table gradients as well (olb_trace_bwd_tables_*)
-                rc = getattr(lib, f"olb_trace_bwd_tables_{ctx.sfx}")(
-                    C.byref(dtab.c), 0, S, C.byref(c_in), C.byref(c_rec), C.byref(c_grec),
-                    C.byref(c_gin) if c_gin is not None else None, C.c_void_p(gpar.data_ptr()),
-                    C.c_void_p(gtab.data_ptr()), n, C.c_uint64(mask & ((1 << 64) - 1)), C.c_void_p(stream))
-            else:
-                rc = getattr(lib, f"olb_trace_bwd_{ctx.sfx}")(
-                    C.byref(dtab.c), 0, S, C.byref(c_in), C.byref(c_rec), C.byref(c_grec),
-                    C.byref(c_gin) if c_gin is not None else None, C.c_void_p(gpar.data_ptr()), n,
-                    C.c_uint64(mask & ((1 << 64) - 1)), C.c_void_p(stream))
+            # polynomial / Zernike / Chebyshev surfaces: table gradients as well (grad_tables)
+            rc = getattr(lib, f"olb_trace_bwd_{ctx.sfx}")(
+                C.byref(dtab.c), 0, S, C.byref(c_in), C.byref(c_rec), C.byref(c_grec),
+                C.byref(c_gin) if c_gin is not None else None, C.c_void_p(gpar.data_ptr()),
+                C.c_void_p(gtab.data_ptr() if gtab is not None else None), n, C.c_uint64(mask & ((1 << 64) - 1)),
+                C.c_void_p(stream))
         _lib.check(rc, f"olb_trace_bwd_{ctx.sfx}")
         for s, spec in enumerate(dtab.table.surfaces):
             if spec.kind == T.GEOM_FORBES_QBFS and len(spec.coefficients):

@@ -21,7 +21,7 @@ import torch
 
 from . import _lib
 from . import table as T
-from .trace import RealRays, _DTYPES, _REC_KEYS, _ptr, _require_cuda
+from .trace import RealRays, _REC_KEYS, _c_records, _out_buffer, _require_cuda, _trace
 
 
 def template_params(table: T.SurfaceTable) -> np.ndarray:
@@ -92,11 +92,10 @@ class BatchedTable:
 
 def trace_batch(btab: BatchedTable, rays: RealRays, rays_per_system: int | None = None, shared_input: bool = False,
                 record: bool = True, moments: bool = False, center=(0.0, 0.0), first: int = 0, last: int | None = None):
-    """olb_trace_batch_*.  ``rays`` holds either B * m launch rays (system b owns [b*m, (b+1)*m)) or, with
-    ``shared_input``, m rays that EVERY system traces.  Returns ``(records, moments)``: records = dict of
+    """All B systems in one launch (OlbTraceCall.rays_per_system).  ``rays`` holds either B * m launch rays
+    (system b owns [b*m, (b+1)*m)) or, with ``shared_input``, m rays that EVERY system traces.  Returns ``(records, moments)``: records = dict of
     (rows, B, m) tensors or None; moments = (B, 8) fp64 tensor or None.  Without records and without
     ``shared_input`` the final state is written back into ``rays`` in place."""
-    lib = btab.lib
     B = btab.n_systems
     n_in = len(rays)
     m = int(rays_per_system) if rays_per_system is not None else (n_in if shared_input else n_in // B)
@@ -104,16 +103,13 @@ def trace_batch(btab: BatchedTable, rays: RealRays, rays_per_system: int | None 
         raise ValueError("ray count does not match rays_per_system x n_systems")
     last = btab.template.num_surfaces if last is None else last
     rows = last - first
-    sfx = _DTYPES[rays.dtype]
+    n = B * m
     flags = 0
     recs, c_rec = None, None
     if record and rows > 0:
-        vec = 4 if rays.dtype == torch.float32 else 2
-        n = B * m
-        stride = (n + 63) // 64 * 64 if n % vec else n      # keeps every row 16-byte aligned
-        buf = torch.empty((8, rows, stride), dtype=rays.dtype, device=rays.device)
+        buf = _out_buffer(8, rows, n, rays.dtype, rays.device)
         recs = {k: buf[j, :, :n].view(rows, B, m) for j, k in enumerate(_REC_KEYS)}
-        c_rec = _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], stride)
+        c_rec = _c_records(buf)
         flags |= _lib.TF_NO_FINAL
     if shared_input:
         flags |= _lib.TF_SHARED_INPUT | _lib.TF_NO_FINAL
@@ -125,11 +121,7 @@ def trace_batch(btab: BatchedTable, rays: RealRays, rays_per_system: int | None 
             flags |= _lib.TF_NO_FINAL
     c_rays = _lib.OlbRays(x=rays.x.data_ptr(), y=rays.y.data_ptr(), z=rays.z.data_ptr(), L=rays.L.data_ptr(),
                           M=rays.M.data_ptr(), N=rays.N.data_ptr(), i=rays.i.data_ptr(), opd=rays.opd.data_ptr())
-    cen = (C.c_double * 2)(float(center[0]), float(center[1]))
-    with torch.cuda.device(rays.device):
-        stream = torch.cuda.current_stream(rays.device).cuda_stream
-        rc = getattr(lib, f"olb_trace_batch_{sfx}")(
-            C.byref(btab.c), first, last, C.byref(c_rays), C.byref(c_rec) if c_rec is not None else None, m, flags,
-            cen, _ptr(mom), None, C.c_void_p(stream))
-    _lib.check(rc, f"olb_trace_batch_{sfx}")
+    # (no status word: out-of-range freeform coordinates are not reported on this path)
+    _trace(btab, rays.device, rays.dtype, first, last, n, flags, rays=c_rays, rec=c_rec, center=center, moments=mom,
+           rays_per_system=m, own_status=False)
     return recs, mom

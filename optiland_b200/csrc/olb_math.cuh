@@ -1117,7 +1117,7 @@ OLB_HD void forbes_q_sum2(const T* b, int nc, T x, T& S, T& dS, T& d2S) {
   else { S = (T)2 * a0; dS = (T)2 * d0; d2S = (T)2 * e0; }
 }
 
-// Table gradients of the polynomial families (olb_trace_bwd_tables_*): per surface two blocks (sag table S, slope table
+// Table gradients of the polynomial families (olb_trace_bwd_* grad_tables): per surface two blocks (sag table S, slope table
 // D) of GT_DIM x GT_DIM doubles, entry (i, j) <-> xn^i yn^j; tables wider than GT_DIM are outside the adjoint's scope.
 enum { GT_DIM = 12, GT_BLOCK = GT_DIM * GT_DIM, GT_PER_SURFACE = 2 * GT_BLOCK };
 
@@ -1220,7 +1220,7 @@ OLB_HD bool surface_backward(const PrepSurface<T>& S, const T* pool, T xg0, T yg
       // slope IS the sag's derivative up to its 1e-12 guards, so the same g serves the normal and the
       // implicit-function theorem).  phi' = c^2 / (2 phi da^2); phi'' = c^4 / 4 (k (na da)^-3/2 + 3 (1 + k) na^-1/2 da^-5/2).
       // Outside the normalisation radius (and for an all-zero coefficient set) the surface is the bare conic, as in the
-      // forward pass.  (POLY: Forbes tables run on the olb_trace_bwd_tables_* variant of the kernel.)
+      // forward pass.  (POLY: Forbes tables run on the grad_tables variant of the kernel.)
       fb_a = S.inv_norm * S.inv_norm;
       const T usq = r2 * fb_a;
       if (S.n_coef > 0 && usq < (T)1) {

@@ -152,7 +152,7 @@ struct PrepResult {
   uint32_t hints = 0;          // HINT_* (launch policy only, never semantics)
   bool bwd_supported = true;   // every surface is covered by surface_backward (olb_math.cuh)
   bool bwd_tables = false;     // ... and some surface is a polynomial / Zernike one: its TABLE gradients are wanted
-                               // (olb_trace_bwd_tables_*)
+                               // (olb_trace_bwd_* grad_tables)
   int total_gslots = 0;        // per-thread gradient accumulator slots the backward kernel needs
   std::string error;
 };
@@ -488,7 +488,7 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
                          o.poly_rows <= 12 && o.poly_cols <= 12;
     const bool kind_ok = o.kind == OLB_GEOM_NOOP || o.kind == OLB_GEOM_PLANE || o.kind == OLB_GEOM_STANDARD ||
                          ((o.kind == OLB_GEOM_EVEN_ASPHERE || o.kind == OLB_GEOM_ODD_ASPHERE) && o.n_coef <= 12) || polyfam;
-    // Forbes Q^bfs: covered by the general (olb_trace_bwd_tables_*) variant of the adjoint kernel, at most 12 terms
+    // Forbes Q^bfs: covered by the general (grad_tables) variant of the adjoint kernel, at most 12 terms
     const bool forbes = o.kind == OLB_GEOM_FORBES_QBFS && tab.surfaces[s].n_coef <= 12;
     if (polyfam || forbes) res.bwd_tables = true;
     if (!(kind_ok || forbes) || o.coating == OLB_COAT_FRESNEL || tab.n_wl != 1)

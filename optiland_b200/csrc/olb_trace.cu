@@ -27,23 +27,15 @@
 
 namespace olb {
 
-#ifndef OLB_BLOCK
-#define OLB_BLOCK 256
-#endif
+static constexpr int BLOCK = 256;
 // Minimum resident CTAs per SM asked of ptxas: 16 bytes of ray state per access (float4 /
 // double2) -> 2 CTAs (<= 128 registers), narrower variants -> 3 CTAs (<= 85 registers).
-#ifdef OLB_MIN_BLOCKS
-template <typename T, int RPT, uint32_t FEAT> struct MinBlocks { static constexpr int v = OLB_MIN_BLOCKS; };
-#else
 template <typename T, int RPT, uint32_t FEAT> struct MinBlocks {
   // polarized: the P matrix lives in shared memory, so both precisions fit 2 CTAs per SM (<= 128 registers)
   static constexpr int v = (FEAT & 8u) ? 2 : ((sizeof(T) * RPT <= 8) ? 3 : 2);
 };
-#endif
-static constexpr int BLOCK = OLB_BLOCK;
-#ifndef OLB_HOST_SLOTS
-#define OLB_HOST_SLOTS 3
-#endif
+// Host-buffer pipeline: chunks in flight (H2D of one overlaps kernel / D2H of the others).
+static constexpr int HOST_SLOTS = 3;
 
 static thread_local std::string g_last_error;
 static std::atomic<int64_t> g_launches{0};
@@ -87,12 +79,12 @@ struct TraceArgs {
   // fused moments epilogue (OLB_TF_MOMENTS)
   double* moments;
   double mcx, mcy;
-  // batched systems (olb_trace_batch_*): blockIdx.y = system, its table at blob + y * blob_stride, its rays
+  // batched systems (OlbTraceCall.rays_per_system): blockIdx.y = system, its table at blob + y * blob_stride, its rays
   // are the segment [y * sys_rays, (y+1) * sys_rays); shared_in: every system reads the SAME sys_rays inputs
   int64_t sys_rays;
   int32_t blob_stride;
   int32_t shared_in;
-  // wavefront epilogue (olb_trace_wavefront_*) when wf_opd != nullptr
+  // wavefront epilogue (OlbTraceCall.wavefront_out) when wf_opd != nullptr
   void* wf_opd; void* wf_px; void* wf_py; void* wf_pz; void* wf_i;
   WavefrontRef wf;
   // polarized intensity epilogue (OlbPolarization): 0 off, 1 one polarized state, 2 unpolarized
@@ -521,13 +513,10 @@ struct BwdArgs {
 // global atomic per slot and CTA)  (ACC == 2).  When the table needs more slots than two resident CTAs can hold that
 // way (fp64 with more than ~50 slots: configuration 3), neighbouring lanes share one accumulator after ONE shuffle
 // (ACC == 1: [slot][thread / 2], half the shared memory); beyond that each surface's contributions are
-// warp-reduced immediately (ACC == 0: five shuffles per value).
-#ifndef OLB_BWD_MINB64
-#define OLB_BWD_MINB64 2
-#endif
+// warp-reduced immediately (ACC == 0: five shuffles per value).  Both precisions ask for 2 resident CTAs per SM.
 // POLY: the table holds polynomial / Zernike surfaces (table gradients wanted); false compiles those paths out.
 template <typename T, int ACC, bool POLY>
-__global__ void __launch_bounds__(BLOCK, (sizeof(T) == 8 ? OLB_BWD_MINB64 : 2)) trace_bwd_kernel(const __grid_constant__ BwdArgs a) {
+__global__ void __launch_bounds__(BLOCK, 2) trace_bwd_kernel(const __grid_constant__ BwdArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem);
   unsigned char* tab = smem + 16;
@@ -747,14 +736,14 @@ __global__ void __launch_bounds__(BLOCK, (sizeof(T) == 8 ? OLB_BWD_MINB64 : 2)) 
 template <typename T>
 static int trace_bwd_impl(const OlbDeviceTable* wh, int32_t first, int32_t last, const OlbRays* rays_in,
                           const OlbRecords* rec, const OlbRecords* grec, const OlbRays* gin, double* gparams,
-                          int64_t n_rays, uint64_t grow_mask, cudaStream_t stream, double* gtab = nullptr) {
+                          double* gtab, int64_t n_rays, uint64_t grow_mask, cudaStream_t stream) {
   if (!wh || wh->magic != WS_MAGIC || !wh->workspace)
     return fail(OLB_ERR_INVALID_ARG, "table handle was not initialised by olb_table_upload");
   if (!wh->bwd_supported)
     return fail(OLB_ERR_UNSUPPORTED, "backward: table not supported (a geometry other than plane / standard / even- and "
                                      "odd-asphere / polynomial / Zernike, a Fresnel coating or several wavelengths)");
   if (wh->bwd_supported == 2 && !gtab)
-    return fail(OLB_ERR_UNSUPPORTED, "backward: the table has polynomial / Zernike surfaces: use olb_trace_bwd_tables_* (grad_tables)");
+    return fail(OLB_ERR_UNSUPPORTED, "backward: the table has polynomial / Zernike surfaces: grad_tables is required");
   if (!rays_in || !rec || !gparams) return fail(OLB_ERR_INVALID_ARG, "rays_in, rec and grad_params are required");
   if (first < 0 || last > wh->n_surfaces || first > last) return fail(OLB_ERR_INVALID_ARG, "bad surface range");
   if (n_rays <= 0 || first == last) return OLB_OK;
@@ -787,9 +776,7 @@ static int trace_bwd_impl(const OlbDeviceTable* wh, int32_t first, int32_t last,
   const size_t smem_warp = base_smem + (size_t)wh->n_surfaces * GP_COUNT * sizeof(double);
   const size_t smem_pair = base_smem + (size_t)wh->bwd_slots * (BLOCK / 2) * sizeof(T);
   // 2 CTAs per SM must still fit: 228 KB per SM, 1 KB of it reserved per resident CTA -> 113 KB each
-  static const int force_acc = [] { const char* e = getenv("OLB_BWD_ACC"); return e ? atoi(e) : -1; }();   // (profiling)
-  int acc = smem_acc <= 113 * 1024 ? 2 : (smem_pair <= 113 * 1024 ? 1 : 0);
-  if (force_acc >= 0 && force_acc < acc) acc = force_acc;
+  const int acc = smem_acc <= 113 * 1024 ? 2 : (smem_pair <= 113 * 1024 ? 1 : 0);
   const bool poly = a.gtab != nullptr;
   auto kern = acc == 2 ? (poly ? trace_bwd_kernel<T, 2, true> : trace_bwd_kernel<T, 2, false>)
             : acc == 1 ? (poly ? trace_bwd_kernel<T, 1, true> : trace_bwd_kernel<T, 1, false>)
@@ -802,8 +789,7 @@ static int trace_bwd_impl(const OlbDeviceTable* wh, int32_t first, int32_t last,
   OLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BLOCK, smem));
   if (per_sm < 1) return fail(OLB_ERR_CUDA, "backward kernel does not fit on an SM");
   // the backward pass is read-dominated: one resident wave is best (measured 1.52 ms vs 1.84 ms at 64x)
-  static const int bwd_mult = [] { const char* e = getenv("OLB_BWD_GRID_MULT"); return e ? atoi(e) : 1; }();
-  int64_t grid = (int64_t)num_sms * per_sm * (bwd_mult > 0 ? bwd_mult : 1);
+  int64_t grid = (int64_t)num_sms * per_sm;
   const int64_t n_tiles = (n_rays + BLOCK - 1) / BLOCK;
   if (grid > n_tiles) grid = n_tiles;
   kern<<<(unsigned)grid, BLOCK, smem, stream>>>(a);
@@ -851,8 +837,7 @@ static int launch_instance(const TraceArgs& a, cudaStream_t stream) {
   // A one-wave persistent grid keeps all CTAs in lock-step (everybody loads, then everybody stores row
   // r ...); staggered CTA start times spread the concurrent write streams.  On an H100 (Double-Gauss,
   // 10 M rays, full records) 64x and 16x tie, 4x and 1x are 3-4 % slower in fp32.
-  static const int grid_mult = [] { const char* e = getenv("OLB_GRID_MULT"); return e ? atoi(e) : 64; }();
-  int64_t grid = (int64_t)num_sms * blocks_per_sm * (grid_mult > 0 ? grid_mult : 1);
+  int64_t grid = (int64_t)num_sms * blocks_per_sm * 64;
   if (grid > n_tiles) grid = n_tiles;
   if (grid < 1) return OLB_OK;
   kern<<<(unsigned)grid, BLOCK, smem, stream>>>(a);
@@ -896,17 +881,26 @@ static int launch_feat_cf(const TraceArgs& a, uint32_t features, cudaStream_t st
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 template <typename T>
-static int trace_impl(const OlbDeviceTable* wh, int32_t first, int32_t last, const OlbRays* rays,
-                      const OlbRecords* rec, int64_t n_rays, uint32_t flags, int32_t* status,
-                      cudaStream_t stream, const OlbPupilLaunch* launch = nullptr, const double* center = nullptr,
-                      double* moments = nullptr, int64_t rays_per_system = 0, const OlbWavefrontRef* wref = nullptr,
-                      const OlbWavefrontOut* wout = nullptr, const OlbPolarization* pol = nullptr) {
+static int trace_impl(const OlbDeviceTable* wh, const OlbTraceCall& c, cudaStream_t stream) {
   if (!wh || wh->magic != WS_MAGIC || !wh->workspace)
     return fail(OLB_ERR_INVALID_ARG, "table handle was not initialised by olb_table_upload");
   const unsigned char* workspace_dev = (const unsigned char*)wh->workspace;
-  if (!rays) return fail(OLB_ERR_INVALID_ARG, "rays is NULL");
+  const int32_t first = c.first, last = c.last;
+  const int64_t n_rays = c.n_rays, rays_per_system = c.rays_per_system;
+  uint32_t flags = c.flags;
+  const OlbPupilLaunch* launch = c.launch;
+  double* moments = c.moments;
+  const OlbWavefrontRef* wref = c.wavefront_ref;
+  const OlbWavefrontOut* wout = c.wavefront_out;
+  const OlbPolarization* pol = c.pol;
+  const OlbRecords* rec = c.rec;
+  const OlbRays none{};
+  const OlbRays* rays = c.rays ? c.rays : &none;   // pupil launch / NO_FINAL: the ray arrays may all be NULL
   if (n_rays < 0) return fail(OLB_ERR_INVALID_ARG, "n_rays < 0");
+  if (rays_per_system < 0) return fail(OLB_ERR_INVALID_ARG, "rays_per_system < 0");
   if (first < 0 || last > wh->n_surfaces || first > last) return fail(OLB_ERR_INVALID_ARG, "bad surface range");
+  if (wh->n_systems > 1 && rays_per_system == 0)
+    return fail(OLB_ERR_INVALID_ARG, "this table holds several systems: set rays_per_system");
   if (n_rays == 0 || first == last) return OLB_OK;
   void* req[] = {rays->x, rays->y, rays->z, rays->L, rays->M, rays->N, rays->i, rays->opd};
   if (moments) flags |= OLB_TF_MOMENTS; else flags &= ~uint32_t(OLB_TF_MOMENTS);
@@ -931,7 +925,7 @@ static int trace_impl(const OlbDeviceTable* wh, int32_t first, int32_t last, con
   a.x = rays->x; a.y = rays->y; a.z = rays->z; a.L = rays->L; a.M = rays->M; a.N = rays->N;
   a.i = rays->i; a.w = rays->w; a.opd = rays->opd;
   a.L0 = rays->L0; a.M0 = rays->M0; a.N0 = rays->N0; a.p = rays->p;
-  a.status = status;
+  a.status = c.status;
   a.tflags = flags;
   if (rays_per_system > 0) {
     if (wh->n_systems < 1 || n_rays != rays_per_system * (int64_t)wh->n_systems)
@@ -942,10 +936,8 @@ static int trace_impl(const OlbDeviceTable* wh, int32_t first, int32_t last, con
     a.shared_in = (flags & OLB_TF_SHARED_INPUT) ? 1 : 0;
     if (a.shared_in && !(flags & OLB_TF_NO_FINAL))
       return fail(OLB_ERR_INVALID_ARG, "OLB_TF_SHARED_INPUT needs OLB_TF_NO_FINAL (results go to records / moments)");
-  } else if (wh->n_systems > 1) {
-    return fail(OLB_ERR_INVALID_ARG, "this table holds several systems: use olb_trace_batch_*");
   }
-  if (moments) { a.moments = moments; a.mcx = center ? center[0] : 0.0; a.mcy = center ? center[1] : 0.0; }
+  if (moments) { a.moments = moments; a.mcx = c.center[0]; a.mcy = c.center[1]; }
   if (wref || wout) {
     if (!wref || !wout) return fail(OLB_ERR_INVALID_ARG, "wavefront: ref and out are both required");
     void* wo[] = {wout->opd, wout->pupil_x, wout->pupil_y, wout->pupil_z, wout->intensity};
@@ -1030,8 +1022,6 @@ static int trace_impl(const OlbDeviceTable* wh, int32_t first, int32_t last, con
   // records traces in 3.25 ms against 3.33 ms with one ray per thread).  Tables with
   // Newton surfaces / aperture programs / coatings: fp32 -> 2, fp64 -> 1 (their per-ray code
   // is large; more rays per thread only spills).
-  // OLB_FORCE_RPT is a tuning knob for benchmarks only.
-  static const int force_rpt = [] { const char* e = getenv("OLB_FORCE_RPT"); return e ? atoi(e) : 0; }();
   if (features & FEAT_POL) {
     if (!(flags & OLB_TF_POLARIZED))
       return fail(OLB_ERR_INVALID_ARG, "table has Fresnel coatings: needs OLB_TF_POLARIZED and rays.p "
@@ -1047,8 +1037,7 @@ static int trace_impl(const OlbDeviceTable* wh, int32_t first, int32_t last, con
   // fp32: 4 rays/thread closed form, 2 with even/odd aspheres, 1 with the polynomial-family Newton surfaces
   // (2 rays/thread only adds register pressure to their long Newton loops)
   const bool poly_newton = (wh->hints & (int32_t)HINT_POLY_NEWTON) != 0;
-  int rpt = force_rpt > 0 ? force_rpt : (sizeof(T) == 4 ? (closed_form ? 4 : (poly_newton ? 1 : 2)) : (closed_form ? 2 : 1));
-  if (!closed_form && rpt > 2) rpt = 2;
+  const int rpt = sizeof(T) == 4 ? (closed_form ? 4 : (poly_newton ? 1 : 2)) : (closed_form ? 2 : 1);
   if constexpr (sizeof(T) == 4) {
     if (rpt >= 4 && vec_ok) return launch_feat_cf<T, 4>(a, features, stream);
     if (rpt >= 2 && rec_stride_ok2) return launch_feat<T, 2>(a, features, stream);
@@ -1169,142 +1158,42 @@ int olb_table_upload_batch(const OlbTable* template_table, const double* params,
   return OLB_OK;
 }
 
-int olb_trace_batch_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays,
-                        const OlbRecords* rec, int64_t rays_per_system, uint32_t flags, const double center[2],
-                        double* moments, int32_t* status, void* stream) {
-  if (!table || rays_per_system < 1) return fail(OLB_ERR_INVALID_ARG, "bad batch arguments");
-  OlbRays none{};
-  return trace_impl<float>(table, first, last, rays ? rays : &none, rec, rays_per_system * table->n_systems, flags, status,
-                           (cudaStream_t)stream, nullptr, center, moments, rays_per_system);
+int olb_trace_call_f32(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream) {
+  if (!call) return fail(OLB_ERR_INVALID_ARG, "call is NULL");
+  return trace_impl<float>(table, *call, (cudaStream_t)stream);
 }
-int olb_trace_batch_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays,
-                        const OlbRecords* rec, int64_t rays_per_system, uint32_t flags, const double center[2],
-                        double* moments, int32_t* status, void* stream) {
-  if (!table || rays_per_system < 1) return fail(OLB_ERR_INVALID_ARG, "bad batch arguments");
-  OlbRays none{};
-  return trace_impl<double>(table, first, last, rays ? rays : &none, rec, rays_per_system * table->n_systems, flags, status,
-                            (cudaStream_t)stream, nullptr, center, moments, rays_per_system);
-}
-
-int olb_trace_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays,
-                  const OlbRecords* rec, int64_t n_rays, uint32_t flags, int32_t* status, void* stream) {
-  return trace_impl<float>(table, first, last, rays, rec, n_rays, flags, status, (cudaStream_t)stream);
-}
-
-int olb_trace_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays,
-                  const OlbRecords* rec, int64_t n_rays, uint32_t flags, int32_t* status, void* stream) {
-  return trace_impl<double>(table, first, last, rays, rec, n_rays, flags, status, (cudaStream_t)stream);
+int olb_trace_call_f64(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream) {
+  if (!call) return fail(OLB_ERR_INVALID_ARG, "call is NULL");
+  return trace_impl<double>(table, *call, (cudaStream_t)stream);
 }
 
 int olb_trace_bwd_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays_in,
                       const OlbRecords* rec, const OlbRecords* grad_rec, const OlbRays* grad_rays_in,
-                      double* grad_params, int64_t n_rays, uint64_t grad_row_mask, void* stream) {
-  return trace_bwd_impl<float>(table, first, last, rays_in, rec, grad_rec, grad_rays_in, grad_params, n_rays,
+                      double* grad_params, double* grad_tables, int64_t n_rays, uint64_t grad_row_mask, void* stream) {
+  return trace_bwd_impl<float>(table, first, last, rays_in, rec, grad_rec, grad_rays_in, grad_params, grad_tables, n_rays,
                                grad_row_mask, (cudaStream_t)stream);
 }
 int olb_trace_bwd_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays_in,
                       const OlbRecords* rec, const OlbRecords* grad_rec, const OlbRays* grad_rays_in,
-                      double* grad_params, int64_t n_rays, uint64_t grad_row_mask, void* stream) {
-  return trace_bwd_impl<double>(table, first, last, rays_in, rec, grad_rec, grad_rays_in, grad_params, n_rays,
+                      double* grad_params, double* grad_tables, int64_t n_rays, uint64_t grad_row_mask, void* stream) {
+  return trace_bwd_impl<double>(table, first, last, rays_in, rec, grad_rec, grad_rays_in, grad_params, grad_tables, n_rays,
                                 grad_row_mask, (cudaStream_t)stream);
 }
 
-int olb_trace_bwd_tables_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays_in,
-                             const OlbRecords* rec, const OlbRecords* grad_rec, const OlbRays* grad_rays_in,
-                             double* grad_params, double* grad_tables, int64_t n_rays, uint64_t grad_row_mask, void* stream) {
-  if (!grad_tables) return fail(OLB_ERR_INVALID_ARG, "grad_tables is NULL");
-  return trace_bwd_impl<float>(table, first, last, rays_in, rec, grad_rec, grad_rays_in, grad_params, n_rays,
-                               grad_row_mask, (cudaStream_t)stream, grad_tables);
-}
-int olb_trace_bwd_tables_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays_in,
-                             const OlbRecords* rec, const OlbRecords* grad_rec, const OlbRays* grad_rays_in,
-                             double* grad_params, double* grad_tables, int64_t n_rays, uint64_t grad_row_mask, void* stream) {
-  if (!grad_tables) return fail(OLB_ERR_INVALID_ARG, "grad_tables is NULL");
-  return trace_bwd_impl<double>(table, first, last, rays_in, rec, grad_rec, grad_rays_in, grad_params, n_rays,
-                                grad_row_mask, (cudaStream_t)stream, grad_tables);
-}
-
-int olb_trace_pupil_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                        const OlbRays* out, const OlbRecords* rec, int64_t n_rays, uint32_t flags, int32_t* status,
-                        void* stream) {
-  if (!launch) return fail(OLB_ERR_INVALID_ARG, "launch is NULL");
-  OlbRays none{};
-  return trace_impl<float>(table, first, last, out ? out : &none, rec, n_rays, flags, status, (cudaStream_t)stream, launch);
-}
-int olb_trace_pupil_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                        const OlbRays* out, const OlbRecords* rec, int64_t n_rays, uint32_t flags, int32_t* status,
-                        void* stream) {
-  if (!launch) return fail(OLB_ERR_INVALID_ARG, "launch is NULL");
-  OlbRays none{};
-  return trace_impl<double>(table, first, last, out ? out : &none, rec, n_rays, flags, status, (cudaStream_t)stream, launch);
-}
-
-int olb_trace_wavefront_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                            const OlbRays* rays, const OlbRecords* rec, int64_t n_rays, uint32_t flags,
-                            const OlbWavefrontRef* ref, const OlbWavefrontOut* out, int32_t* status, void* stream) {
-  if (!ref || !out) return fail(OLB_ERR_INVALID_ARG, "wavefront: ref / out is NULL");
-  OlbRays none{};
-  return trace_impl<float>(table, first, last, rays ? rays : &none, rec, n_rays, flags, status, (cudaStream_t)stream,
-                           launch, nullptr, nullptr, 0, ref, out);
-}
-int olb_trace_wavefront_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                            const OlbRays* rays, const OlbRecords* rec, int64_t n_rays, uint32_t flags,
-                            const OlbWavefrontRef* ref, const OlbWavefrontOut* out, int32_t* status, void* stream) {
-  if (!ref || !out) return fail(OLB_ERR_INVALID_ARG, "wavefront: ref / out is NULL");
-  OlbRays none{};
-  return trace_impl<double>(table, first, last, rays ? rays : &none, rec, n_rays, flags, status, (cudaStream_t)stream,
-                            launch, nullptr, nullptr, 0, ref, out);
-}
-
-int olb_trace_polarized_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                            const OlbRays* rays, const OlbRecords* rec, int64_t n_rays, uint32_t flags,
-                            const OlbPolarization* pol, const OlbWavefrontRef* ref, const OlbWavefrontOut* out,
-                            int32_t* status, void* stream) {
-  OlbRays none{};
-  return trace_impl<float>(table, first, last, rays ? rays : &none, rec, n_rays, flags | OLB_TF_POLARIZED, status,
-                           (cudaStream_t)stream, launch, nullptr, nullptr, 0, ref, out, pol);
-}
-int olb_trace_polarized_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                            const OlbRays* rays, const OlbRecords* rec, int64_t n_rays, uint32_t flags,
-                            const OlbPolarization* pol, const OlbWavefrontRef* ref, const OlbWavefrontOut* out,
-                            int32_t* status, void* stream) {
-  OlbRays none{};
-  return trace_impl<double>(table, first, last, rays ? rays : &none, rec, n_rays, flags | OLB_TF_POLARIZED, status,
-                            (cudaStream_t)stream, launch, nullptr, nullptr, 0, ref, out, pol);
-}
-
-int olb_trace_moments_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                          const OlbRays* rays, const OlbRecords* rec, int64_t n_rays, uint32_t flags,
-                          const double center[2], double* moments, int32_t* status, void* stream) {
-  if (!moments) return fail(OLB_ERR_INVALID_ARG, "moments is NULL");
-  OlbRays none{};
-  return trace_impl<float>(table, first, last, rays ? rays : &none, rec, n_rays, flags, status, (cudaStream_t)stream,
-                           launch, center, moments);
-}
-int olb_trace_moments_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                          const OlbRays* rays, const OlbRecords* rec, int64_t n_rays, uint32_t flags,
-                          const double center[2], double* moments, int32_t* status, void* stream) {
-  if (!moments) return fail(OLB_ERR_INVALID_ARG, "moments is NULL");
-  OlbRays none{};
-  return trace_impl<double>(table, first, last, rays ? rays : &none, rec, n_rays, flags, status, (cudaStream_t)stream,
-                            launch, center, moments);
-}
-
 // ---- host-buffer end-to-end path ---------------------------------------------------------------
-// scratch layout: OLB_HOST_SLOTS slots x 9 arrays (x,y,z,L,M,N,i,w,opd) x chunk elements
+// scratch layout: HOST_SLOTS slots x 9 arrays (x,y,z,L,M,N,i,w,opd) x chunk elements
 int64_t olb_host_scratch_bytes(int32_t elem_size, int64_t chunk_rays) {
   if ((elem_size != 4 && elem_size != 8) || chunk_rays < 1) return fail(OLB_ERR_INVALID_ARG, "bad scratch query");
   const int64_t chunk_al = (chunk_rays + 63) & ~int64_t(63);
-  return (int64_t)OLB_HOST_SLOTS * 9 * chunk_al * elem_size;
+  return (int64_t)HOST_SLOTS * 9 * chunk_al * elem_size;
 }
 
 }  // extern "C"
 
 template <typename T>
-static int trace_host_impl(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* h_in,
-                           const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays, int64_t chunk,
-                           void* scratch, int64_t scratch_bytes, uint32_t flags, int32_t* status,
-                           const OlbPupilLaunch* launch = nullptr) {
+static int trace_host_impl(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
+                           const OlbRays* h_in, const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays,
+                           int64_t chunk, void* scratch, int64_t scratch_bytes, uint32_t flags, int32_t* status) {
   if (!table || table->magic != WS_MAGIC) return fail(OLB_ERR_INVALID_ARG, "table handle was not initialised");
   const OlbDeviceTable& wh = *table;
   OlbRays pupil_in{};
@@ -1330,7 +1219,7 @@ static int trace_host_impl(const OlbDeviceTable* table, int32_t first, int32_t l
   if (need_w && !in[7]) return fail(OLB_ERR_INVALID_ARG, "h_in.w is NULL but the table has several wavelengths");
 
   const int64_t chunk_al = (chunk + 63) & ~int64_t(63);
-  constexpr int NS = OLB_HOST_SLOTS;   // chunks in flight: H2D of one overlaps kernel / D2H of the others
+  constexpr int NS = HOST_SLOTS;
   T* slot[NS][9];
   for (int s = 0; s < NS; ++s)
     for (int k = 0; k < 9; ++k) slot[s][k] = (T*)scratch + ((int64_t)s * 9 + k) * chunk_al;
@@ -1386,8 +1275,10 @@ static int trace_host_impl(const OlbDeviceTable* table, int32_t first, int32_t l
       dl.Py = slot[s][1];
       if (per_ray_fields) { dl.Hx = slot[s][2]; dl.Hy = slot[s][3]; }   // (read by each thread before it writes z / L)
     }
-    result = trace_impl<T>(&wh, first, last, &d, rp, m, flags & ~uint32_t(OLB_TF_NO_FINAL), status, q,
-                           launch ? &dl : nullptr);
+    OlbTraceCall call{};
+    call.first = first; call.last = last; call.n_rays = m; call.flags = flags & ~uint32_t(OLB_TF_NO_FINAL);
+    call.rays = &d; call.rec = rp; call.launch = launch ? &dl : nullptr; call.status = status;
+    result = trace_impl<T>(&wh, call, q);
     if (result) break;
     for (int k = 0; k < 9; ++k) {
       if (k == 7) continue;
@@ -1407,31 +1298,17 @@ static int trace_host_impl(const OlbDeviceTable* table, int32_t first, int32_t l
 
 extern "C" {
 
-int olb_trace_host_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* h_in,
-                       const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
-                       void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags, int32_t* status) {
-  return trace_host_impl<float>(table, first, last, h_in, h_out, rec, n_rays, chunk_rays, dev_scratch,
+int olb_trace_host_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
+                       const OlbRays* h_in, const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays,
+                       int64_t chunk_rays, void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags, int32_t* status) {
+  return trace_host_impl<float>(table, first, last, launch, h_in, h_out, rec, n_rays, chunk_rays, dev_scratch,
                                 dev_scratch_bytes, flags, status);
 }
-int olb_trace_host_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* h_in,
-                       const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
-                       void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags, int32_t* status) {
-  return trace_host_impl<double>(table, first, last, h_in, h_out, rec, n_rays, chunk_rays, dev_scratch,
+int olb_trace_host_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
+                       const OlbRays* h_in, const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays,
+                       int64_t chunk_rays, void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags, int32_t* status) {
+  return trace_host_impl<double>(table, first, last, launch, h_in, h_out, rec, n_rays, chunk_rays, dev_scratch,
                                  dev_scratch_bytes, flags, status);
-}
-int olb_trace_host_pupil_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                             const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
-                             void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags, int32_t* status) {
-  if (!launch) return fail(OLB_ERR_INVALID_ARG, "launch is NULL");
-  return trace_host_impl<float>(table, first, last, nullptr, h_out, rec, n_rays, chunk_rays, dev_scratch,
-                                dev_scratch_bytes, flags, status, launch);
-}
-int olb_trace_host_pupil_f64(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbPupilLaunch* launch,
-                             const OlbRays* h_out, const OlbRecords* rec, int64_t n_rays, int64_t chunk_rays,
-                             void* dev_scratch, int64_t dev_scratch_bytes, uint32_t flags, int32_t* status) {
-  if (!launch) return fail(OLB_ERR_INVALID_ARG, "launch is NULL");
-  return trace_host_impl<double>(table, first, last, nullptr, h_out, rec, n_rays, chunk_rays, dev_scratch,
-                                 dev_scratch_bytes, flags, status, launch);
 }
 
 }  // extern "C"

@@ -231,10 +231,10 @@ class CudaEngine:
         return torch.is_tensor(t) and t.is_cuda and t.dtype in (torch.float32, torch.float64) and t.ndim == 1
 
     def trace_pupil(self, table: T.SurfaceTable, Px, Py, affine: dict, wavelength=None, polarization=False):
-        """Launch state generated in-kernel from the pupil samples (olb_trace_pupil_*; with ``affine["fields"]``
+        """Launch state generated in-kernel from the pupil samples (OlbTraceCall.launch; with ``affine["fields"]``
         also from per-ray field points).  ``wavelength``: per-ray array for a multi-wavelength table.  Returns the
         record dict; the final state is its last row.  ``polarization``: False, or the optic's polarization state
-        (None = unpolarized, or (Ex, Ey, phase_x, phase_y)) -- PolarizedRays are traced (olb_trace_polarized_*) and
+        (None = unpolarized, or (Ex, Ey, phase_x, phase_y)) -- PolarizedRays are traced (OLB_TF_POLARIZED, OlbTraceCall.pol) and
         the dict also holds ``"p"`` (the (N, 3, 3) complex matrices) and ``"i_pol"`` (update_intensity's result)."""
         from .trace import trace_pupil_device
 
@@ -251,7 +251,7 @@ class CudaEngine:
 
     def trace_wavefront(self, table: T.SurfaceTable, Px, Py, affine: dict, ref: dict, polarized: bool = False) -> dict:
         """One field's pupil grid -> OPD map + exit-pupil intercepts + intensity, nothing else written
-        (olb_trace_wavefront_*); ``polarized``: PolarizedRays, the result also holds the P matrices ``"p"``."""
+        (OlbTraceCall.wavefront_*); ``polarized``: PolarizedRays, the result also holds the P matrices ``"p"``."""
         from .trace import trace_wavefront_device
 
         dt = self.device_table(table, Px.device)
@@ -260,7 +260,7 @@ class CudaEngine:
 
     def spot_moments(self, table: T.SurfaceTable, Px, Py, affine: dict, center=(0.0, 0.0), last=None,
                      global_xy: bool = False, every_ray: bool = False) -> list:
-        """Launch generation + trace + moment sums in ONE kernel, nothing written per ray (olb_trace_moments_*):
+        """Launch generation + trace + moment sums in ONE kernel, nothing written per ray (OlbTraceCall.moments):
         the 8 sums of include/olb.h as Python floats (one 64-byte read-back)."""
         from .trace import trace_moments_device
 
@@ -670,7 +670,7 @@ def _live_params(surfaces, table, wavelength):
 def _live_coefs(surfaces, table):
     """(S, K) fp64 tensor of the USER coefficients of the polynomial-family surfaces (Zernike ``geometry.zernike.coeffs``,
     polynomial / Chebyshev ``geometry.coefficients``), stacked from the LIVE tensors so that the table gradients of
-    olb_trace_bwd_tables_* flow back to the optimiser's variables (optimization/variable/zernike_coeff.py,
+    olb_trace_bwd_* (grad_tables) flow back to the optimiser's variables (optimization/variable/zernike_coeff.py,
     polynomial_coeff.py, chebyshev_coeff.py); None when the table has no such surface."""
     import torch
 

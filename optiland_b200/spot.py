@@ -1,5 +1,5 @@
 """SURVEY.md 8f-2 wired into the reference's classes: spot STATISTICS from the fused moments epilogue
-(olb_trace_moments_*) -- launch generation + trace + moment sums in one kernel, nothing written per ray -- behind
+(OlbTraceCall.moments) -- launch generation + trace + moment sums in one kernel, nothing written per ray -- behind
 
 * ``RayOperand.rms_spot_size``        optiland/optimization/operand/ray.py:299-342
 * ``SpotDiagram.rms_spot_radius`` / ``.centroid``   optiland/analysis/spot_diagram/core.py:329-370
@@ -42,7 +42,7 @@ class LazySpotData:
 
     # ---- statistics without per-ray data ---------------------------------------------------------------
     def moments(self, center=(0.0, 0.0)):
-        """8 moment sums of the masked (i > 0) intercepts about ``center`` (include/olb.h: olb_trace_moments_*), in the
+        """8 moment sums of the masked (i > 0) intercepts about ``center`` (include/olb.h: OlbTraceCall.moments), in the
         image surface's local frame or in global coordinates, as the SpotDiagram was configured."""
         key = (float(center[0]), float(center[1]))
         m = self._moments.get(key)

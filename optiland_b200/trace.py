@@ -23,6 +23,7 @@ from . import table as T
 
 _REC_KEYS = ("x", "y", "z", "L", "M", "N", "intensity", "opd")
 _DTYPES = {torch.float32: "f32", torch.float64: "f64"}
+_CDTYPES = {torch.float32: torch.complex64, torch.float64: torch.complex128}
 
 
 def _require_cuda():
@@ -147,8 +148,12 @@ class DeviceTable:
         return int(self.c.features)
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+def _byref(s):
+    return C.byref(s) if s is not None else None
+
+
+def _pointer(s):
+    return C.pointer(s) if s is not None else None
 
 
 def _status_word(dtab: "DeviceTable", device, force: bool = False):
@@ -177,6 +182,53 @@ def _raise_status(status) -> None:
         raise ValueError("k-vector parallel to x-axis is not currently supported.")
 
 
+def _out_buffer(k: int, rows: int, n: int, dtype, device) -> torch.Tensor:
+    """Uninitialised (k, rows, stride) output rows of n rays.  The kernel uses vector accesses (4 fp32 / 2 fp64 rays)
+    only when every row starts on a vector boundary, so the stride is n when n is a multiple of the vector width and
+    otherwise n rounded up to 64 (every row stays 16-byte aligned)."""
+    vec = 4 if dtype == torch.float32 else 2
+    stride = n if n % vec == 0 else (n + 63) // 64 * 64
+    return torch.empty((k, rows, stride), dtype=dtype, device=device)
+
+
+def _c_records(buf: torch.Tensor):
+    """OlbRecords over an (8, rows, stride) buffer."""
+    return _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], buf.shape[-1])
+
+
+def _take_last_row(rays, recs):
+    """``rays.x`` .. ``rays.opd`` become views of the last record row (with OLB_TF_NO_FINAL the kernel writes the
+    final state only there)."""
+    rays.x, rays.y, rays.z = recs["x"][-1], recs["y"][-1], recs["z"][-1]
+    rays.L, rays.M, rays.N = recs["L"][-1], recs["M"][-1], recs["N"][-1]
+    rays.i, rays.opd = recs["intensity"][-1], recs["opd"][-1]
+    return rays
+
+
+def _trace(dtab, device, dtype, first, last, n, flags, rays=None, rec=None, launch=None, center=(0.0, 0.0),
+           moments=None, rays_per_system=0, wavefront=None, pol=None, status=None, own_status=True):
+    """The one forward call of the library (olb_trace_call_f32 / _f64, include/olb.h: OlbTraceCall).  ``rays`` /
+    ``rec`` / ``launch`` / ``pol``: ctypes structs or None; ``wavefront``: (OlbWavefrontRef, OlbWavefrontOut) or None;
+    ``moments``: device tensor or None.  ``own_status``: the status word is made here (when the table or the call
+    shape can set OLB_ST_* bits) and the reference's errors are raised from it; otherwise ``status`` (a caller-owned
+    device int32, or None) is passed through unchecked."""
+    if own_status:
+        status = _status_word(dtab, device, force=pol is not None)
+    ref, out = wavefront if wavefront is not None else (None, None)
+    call = _lib.OlbTraceCall(
+        first=first, last=last, n_rays=n, flags=flags, rays=_pointer(rays), rec=_pointer(rec), launch=_pointer(launch),
+        center=(float(center[0]), float(center[1])), moments=moments.data_ptr() if moments is not None else None,
+        rays_per_system=rays_per_system, wavefront_ref=_pointer(ref), wavefront_out=_pointer(out), pol=_pointer(pol),
+        status=status.data_ptr() if status is not None else None)
+    sfx = _DTYPES[dtype]
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device).cuda_stream
+        rc = getattr(dtab.lib, f"olb_trace_call_{sfx}")(C.byref(dtab.c), C.byref(call), C.c_void_p(stream))
+    _lib.check(rc, f"olb_trace_call_{sfx}")
+    if own_status:
+        _raise_status(status)
+
+
 def _c_polarization(state, intensity_out=None):
     """OlbPolarization from ``state`` = None / "unpolarized" (the mean of two orthogonal states) or
     (Ex, Ey, phase_x, phase_y) (normalised as PolarizationState does, polarization_state.py:53-56)."""
@@ -193,7 +245,7 @@ def _c_polarization(state, intensity_out=None):
 
 def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, record: bool = True,
                  want_l0: bool = False, polarization=False):
-    """One call of olb_trace_f32/f64.  Returns the dict of (rows, N) record tensors (or None).
+    """One trace of ``rays`` on the device.  Returns the dict of (rows, N) record tensors (or None).
 
     With ``record`` the final state is NOT written a second time: ``rays.x`` .. ``rays.opd``
     become views of the last record row (OLB_TF_NO_FINAL), saving 32-64 B/ray of HBM traffic.
@@ -201,13 +253,10 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
     aliasing is not observable through its API.
 
     ``polarization`` (PolarizedRays only): None / "unpolarized" / (Ex, Ey, phase_x, phase_y) runs
-    PolarizedRays.update_intensity as the kernel's epilogue (olb_trace_polarized_*): ``rays.i`` becomes
+    PolarizedRays.update_intensity as the kernel's epilogue (OlbTraceCall.pol): ``rays.i`` becomes
     sum |P E0|^2 i0 / n_states while the record rows keep the geometric intensity.
     """
-    lib = dtab.lib
     n = len(rays)
-    sfx = _DTYPES[rays.dtype]
-    fn = getattr(lib, f"olb_trace_{sfx}")
     if rays.device != dtab.device:
         raise ValueError(f"rays on {rays.device}, table on {dtab.device}")
     rows = last - first
@@ -215,11 +264,9 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
     c_rec = None
     flags = 0
     if record and rows > 0:
-        vec = 4 if rays.dtype == torch.float32 else 2
-        stride = (n + 63) // 64 * 64 if n % vec else n
-        buf = torch.empty((8, rows, stride), dtype=rays.dtype, device=rays.device)
+        buf = _out_buffer(8, rows, n, rays.dtype, rays.device)
         recs = {k: buf[j, :, :n] for j, k in enumerate(_REC_KEYS)}
-        c_rec = _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], stride)
+        c_rec = _c_records(buf)
         flags |= _lib.TF_NO_FINAL
     if want_l0:
         rays.L0 = torch.empty_like(rays.x)
@@ -228,12 +275,11 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
     p_ptr = None
     if isinstance(rays, PolarizedRays):
         flags |= _lib.TF_POLARIZED
-        cdt = torch.complex64 if rays.dtype == torch.float32 else torch.complex128
         if rays.p is None:
-            rays.p = torch.empty((n, 3, 3), dtype=cdt, device=rays.device)
+            rays.p = torch.empty((n, 3, 3), dtype=_CDTYPES[rays.dtype], device=rays.device)
             flags |= _lib.TF_POL_IDENTITY
         else:
-            rays.p = rays.p.to(cdt).contiguous()
+            rays.p = rays.p.to(_CDTYPES[rays.dtype]).contiguous()
         p_ptr = torch.view_as_real(rays.p).data_ptr()
     c_rays = _lib.OlbRays(
         x=rays.x.data_ptr(), y=rays.y.data_ptr(), z=rays.z.data_ptr(), L=rays.L.data_ptr(),
@@ -247,22 +293,9 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
             raise ValueError("the intensity epilogue needs PolarizedRays")
         pol_i = torch.empty_like(rays.x)
         c_pol = _c_polarization(polarization, pol_i)
-    status = _status_word(dtab, rays.device, force=c_pol is not None)
-    with torch.cuda.device(rays.device):
-        stream = torch.cuda.current_stream(rays.device).cuda_stream
-        if c_pol is not None:
-            rc = getattr(lib, f"olb_trace_polarized_{sfx}")(
-                C.byref(dtab.c), first, last, None, C.byref(c_rays), C.byref(c_rec) if c_rec is not None else None,
-                n, flags, C.byref(c_pol), None, None, _ptr(status), C.c_void_p(stream))
-        else:
-            rc = fn(C.byref(dtab.c), first, last, C.byref(c_rays), C.byref(c_rec) if c_rec is not None else None,
-                    n, flags, _ptr(status), C.c_void_p(stream))
-    _lib.check(rc, f"olb_trace_{sfx}")
-    _raise_status(status)
+    _trace(dtab, rays.device, rays.dtype, first, last, n, flags, rays=c_rays, rec=c_rec, pol=c_pol)
     if recs is not None:
-        rays.x, rays.y, rays.z = recs["x"][-1], recs["y"][-1], recs["z"][-1]
-        rays.L, rays.M, rays.N = recs["L"][-1], recs["M"][-1], recs["N"][-1]
-        rays.i, rays.opd = recs["intensity"][-1], recs["opd"][-1]
+        _take_last_row(rays, recs)
     if pol_i is not None:
         rays.i = pol_i
     return recs
@@ -307,82 +340,38 @@ def _c_launch(affine: dict, Px, Py):
 
 def trace_pupil_device(dtab: DeviceTable, Px: torch.Tensor, Py: torch.Tensor, affine: dict, first: int, last: int,
                        wavelength: torch.Tensor | None = None, polarization=False):
-    """olb_trace_pupil_*: launch state generated in-kernel from pupil coordinates (one field), full
-    records.  Returns (rays, records): ``rays`` is a ``RealRays`` view of the last record row.
+    """Launch state generated in-kernel from pupil coordinates (OlbTraceCall.launch, one field or per-ray fields),
+    full records.  Returns (rays, records): ``rays`` is a ``RealRays`` view of the last record row.
 
-    ``polarization`` (config 5's call shape, olb_trace_polarized_*): False = RealRays; otherwise PolarizedRays are
+    ``polarization`` (config 5's call shape): False = RealRays; otherwise PolarizedRays are
     traced -- "matrix": only the P matrices (``rays.p``); None / "unpolarized" / (Ex, Ey, phase_x, phase_y): also the
     intensity epilogue of RealRayTracer.trace in-kernel, ``rays.i`` = sum |P E0|^2 i0 / n_states (the record rows keep
     the geometric intensity, as in the reference)."""
     Px, Py, wavelength = _aligned(Px), _aligned(Py), _aligned(wavelength)
     if affine.get("fields") is not None:
         affine = dict(affine, fields=tuple(_aligned(t) for t in affine["fields"]))
-    if polarization is not False:
-        return _trace_pupil_polarized(dtab, Px, Py, affine, first, last, wavelength, polarization)
-    lib = dtab.lib
-    n = Px.numel()
-    dtype = Px.dtype
-    sfx = _DTYPES[dtype]
-    rows = last - first
-    vec = 4 if dtype == torch.float32 else 2
-    stride = (n + 63) // 64 * 64 if n % vec else n
-    buf = torch.empty((8, rows, stride), dtype=dtype, device=Px.device)
+    n, dtype, dev = Px.numel(), Px.dtype, Px.device
+    buf = _out_buffer(8, last - first, n, dtype, dev)
     recs = {k: buf[j, :, :n] for j, k in enumerate(_REC_KEYS)}
-    c_rec = _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], stride)
     la = _c_launch(affine, Px.contiguous(), Py.contiguous())
     out = _lib.OlbRays(w=wavelength.data_ptr() if (wavelength is not None and dtab.table.n_wl > 1) else None)
-    status = _status_word(dtab, Px.device)
-    with torch.cuda.device(Px.device):
-        stream = torch.cuda.current_stream(Px.device).cuda_stream
-        rc = getattr(lib, f"olb_trace_pupil_{sfx}")(C.byref(dtab.c), first, last, C.byref(la), C.byref(out),
-                                                    C.byref(c_rec), n, _lib.TF_NO_FINAL, _ptr(status), C.c_void_p(stream))
-    _lib.check(rc, f"olb_trace_pupil_{sfx}")
-    _raise_status(status)
-    rays = RealRays.__new__(RealRays)
-    rays.x, rays.y, rays.z = recs["x"][-1], recs["y"][-1], recs["z"][-1]
-    rays.L, rays.M, rays.N = recs["L"][-1], recs["M"][-1], recs["N"][-1]
-    rays.i, rays.opd = recs["intensity"][-1], recs["opd"][-1]
+    flags = _lib.TF_NO_FINAL
+    p, inten, c_pol = None, None, None
+    if polarization is not False:
+        flags |= _lib.TF_POLARIZED
+        p = torch.empty((n, 3, 3), dtype=_CDTYPES[dtype], device=dev)
+        out.p = torch.view_as_real(p).data_ptr()
+        if polarization != "matrix":
+            inten = torch.empty(n, dtype=dtype, device=dev)
+            c_pol = _c_polarization(polarization, inten)
+    _trace(dtab, dev, dtype, first, last, n, flags, rays=out, rec=_c_records(buf), launch=la, pol=c_pol)
+    cls = RealRays if p is None else PolarizedRays
+    rays = _take_last_row(cls.__new__(cls), recs)
+    if p is not None:
+        rays.p = p
+    if inten is not None:
+        rays.i = inten
     rays.w = wavelength
-    rays.L0 = rays.M0 = rays.N0 = None
-    rays.is_normalized = True
-    return rays, recs
-
-
-def _trace_pupil_polarized(dtab, Px, Py, affine, first, last, wavelength, polarization):
-    lib = dtab.lib
-    n = Px.numel()
-    dtype = Px.dtype
-    sfx = _DTYPES[dtype]
-    rows = last - first
-    vec = 4 if dtype == torch.float32 else 2
-    stride = (n + 63) // 64 * 64 if n % vec else n
-    buf = torch.empty((8, rows, stride), dtype=dtype, device=Px.device)
-    recs = {k: buf[j, :, :n] for j, k in enumerate(_REC_KEYS)}
-    c_rec = _lib.OlbRecords(*[buf[j].data_ptr() for j in range(8)], stride)
-    la = _c_launch(affine, Px.contiguous(), Py.contiguous())
-    cdt = torch.complex64 if dtype == torch.float32 else torch.complex128
-    p = torch.empty((n, 3, 3), dtype=cdt, device=Px.device)
-    out = _lib.OlbRays(w=wavelength.data_ptr() if (wavelength is not None and dtab.table.n_wl > 1) else None,
-                       p=torch.view_as_real(p).data_ptr())
-    inten, c_pol = None, None
-    if polarization != "matrix":
-        inten = torch.empty(n, dtype=dtype, device=Px.device)
-        c_pol = _c_polarization(polarization, inten)
-    status = _status_word(dtab, Px.device, force=c_pol is not None)
-    with torch.cuda.device(Px.device):
-        stream = torch.cuda.current_stream(Px.device).cuda_stream
-        rc = getattr(lib, f"olb_trace_polarized_{sfx}")(
-            C.byref(dtab.c), first, last, C.byref(la), C.byref(out), C.byref(c_rec), n, _lib.TF_NO_FINAL,
-            C.byref(c_pol) if c_pol is not None else None, None, None, _ptr(status), C.c_void_p(stream))
-    _lib.check(rc, f"olb_trace_polarized_{sfx}")
-    _raise_status(status)
-    rays = PolarizedRays.__new__(PolarizedRays)
-    rays.x, rays.y, rays.z = recs["x"][-1], recs["y"][-1], recs["z"][-1]
-    rays.L, rays.M, rays.N = recs["L"][-1], recs["M"][-1], recs["N"][-1]
-    rays.i = inten if inten is not None else recs["intensity"][-1]
-    rays.opd = recs["opd"][-1]
-    rays.w = wavelength
-    rays.p = p
     rays.L0 = rays.M0 = rays.N0 = None
     rays.is_normalized = True
     return rays, recs
@@ -393,18 +382,13 @@ WAVEFRONT_KEYS = ("opd", "pupil_x", "pupil_y", "pupil_z", "intensity")
 
 def trace_wavefront_device(dtab: DeviceTable, Px: torch.Tensor, Py: torch.Tensor, affine: dict, ref: dict,
                            wavelength: torch.Tensor | None = None, polarized: bool = False) -> dict:
-    """olb_trace_wavefront_*: trace one field's pupil grid and write ONLY the wavefront data -- OPD in waves
+    """Trace one field's pupil grid and write ONLY the wavefront data (OlbTraceCall.wavefront_*) -- OPD in waves
     against the spherical reference ``ref`` = {center (3), radius, n_image, tilt (2), opd_ref, wavelength_um},
     the exit-pupil intercepts and the image-surface intensity -- no records, no final state
     (optiland/wavefront/strategy.py:152-213).  Returns {key: (N,) tensor} for WAVEFRONT_KEYS."""
     Px, Py, wavelength = _aligned(Px), _aligned(Py), _aligned(wavelength)
-    lib = dtab.lib
-    n = Px.numel()
-    dtype = Px.dtype
-    sfx = _DTYPES[dtype]
-    vec = 4 if dtype == torch.float32 else 2
-    stride = (n + 63) // 64 * 64 if n % vec else n          # keeps every output row 16-byte aligned
-    buf = torch.empty((5, stride), dtype=dtype, device=Px.device)
+    n, dtype, dev = Px.numel(), Px.dtype, Px.device
+    buf = _out_buffer(5, 1, n, dtype, dev)[:, 0]
     c_out = _lib.OlbWavefrontOut(*[buf[j].data_ptr() for j in range(5)])
     c_ref = _lib.OlbWavefrontRef()
     c_ref.center = (C.c_double * 3)(*[float(v) for v in ref["center"]])
@@ -413,26 +397,16 @@ def trace_wavefront_device(dtab: DeviceTable, Px: torch.Tensor, Py: torch.Tensor
     c_ref.opd_ref, c_ref.wavelength_um = float(ref["opd_ref"]), float(ref["wavelength_um"])
     la = _c_launch(affine, Px.contiguous(), Py.contiguous())
     rays = _lib.OlbRays(w=wavelength.data_ptr() if (wavelength is not None and dtab.table.n_wl > 1) else None)
-    status = _status_word(dtab, Px.device)
+    flags = _lib.TF_NO_FINAL
     p = None
-    with torch.cuda.device(Px.device):
-        stream = torch.cuda.current_stream(Px.device).cuda_stream
-        if polarized:
-            # PolarizedRays through the wavefront epilogue (config 5).  The strategy reads the GEOMETRIC intensity
-            # of the image-surface record (wavefront/strategy.py:181) -- no intensity epilogue -- and hands the
-            # polarization ray-tracing matrices on (strategy.py:197-203): `p` is written, 5 + 18 values per ray.
-            cdt = torch.complex64 if dtype == torch.float32 else torch.complex128
-            p = torch.empty((n, 3, 3), dtype=cdt, device=Px.device)
-            rays.p = torch.view_as_real(p).data_ptr()
-            rc = getattr(lib, f"olb_trace_polarized_{sfx}")(
-                C.byref(dtab.c), 0, dtab.table.num_surfaces, C.byref(la), C.byref(rays), None, n, _lib.TF_NO_FINAL,
-                None, C.byref(c_ref), C.byref(c_out), _ptr(status), C.c_void_p(stream))
-        else:
-            rc = getattr(lib, f"olb_trace_wavefront_{sfx}")(
-                C.byref(dtab.c), 0, dtab.table.num_surfaces, C.byref(la), C.byref(rays), None, n, _lib.TF_NO_FINAL,
-                C.byref(c_ref), C.byref(c_out), _ptr(status), C.c_void_p(stream))
-    _lib.check(rc, f"olb_trace_wavefront_{sfx}")
-    _raise_status(status)
+    if polarized:
+        # PolarizedRays through the wavefront epilogue (config 5).  The strategy reads the GEOMETRIC intensity
+        # of the image-surface record (wavefront/strategy.py:181) -- no intensity epilogue -- and hands the
+        # polarization ray-tracing matrices on (strategy.py:197-203): `p` is written, 5 + 18 values per ray.
+        flags |= _lib.TF_POLARIZED
+        p = torch.empty((n, 3, 3), dtype=_CDTYPES[dtype], device=dev)
+        rays.p = torch.view_as_real(p).data_ptr()
+    _trace(dtab, dev, dtype, 0, dtab.table.num_surfaces, n, flags, rays=rays, launch=la, wavefront=(c_ref, c_out))
     out = {k: buf[j, :n] for j, k in enumerate(WAVEFRONT_KEYS)}
     if p is not None:
         out["p"] = p
@@ -443,18 +417,13 @@ def trace_moments_device(dtab: DeviceTable, n: int, dtype, rays: RealRays | None
                          center=(0.0, 0.0), moments: torch.Tensor | None = None, wavelength=None,
                          status: torch.Tensor | None = None, last: int | None = None, global_xy: bool = False,
                          every_ray: bool = False) -> torch.Tensor:
-    """olb_trace_moments_*: trace WITHOUT writing any per-ray output and accumulate the spot / OPD moments
-    of the image-surface intercepts in-kernel (8 fp64 values on the device; see include/olb.h).  Either
+    """Trace WITHOUT writing any per-ray output and accumulate the spot / OPD moments of the image-surface
+    intercepts in-kernel (8 fp64 values on the device; include/olb.h, OlbTraceCall.moments).  Either
     ``rays`` (launch-state arrays, left untouched) or ``pupil`` = (Px, Py, affine).  ``last``: stop after surface
     ``last - 1`` (the moments are of THAT surface); ``global_xy`` / ``every_ray``: OLB_TF_MOMENTS_GLOBAL / _ALL.  ``status``: a caller-owned
     device int32 for the OLB_ST_* bits (a caller that pipelines several launches checks it once at the end with
     ``_raise_status``); by default one is made and checked here for tables that can raise them."""
-    lib = dtab.lib
-    sfx = _DTYPES[dtype]
     dev = dtab.device
-    own_status = status is None
-    if own_status:
-        status = _status_word(dtab, dev)
     if moments is None:
         moments = torch.zeros(8, dtype=torch.float64, device=dev)
     la = None
@@ -471,16 +440,9 @@ def trace_moments_device(dtab: DeviceTable, n: int, dtype, rays: RealRays | None
             setattr(c_rays, k, getattr(rays, k).data_ptr())
         if dtab.table.n_wl > 1:
             c_rays.w = rays.w.data_ptr()
-    cen = (C.c_double * 2)(float(center[0]), float(center[1]))
     flags = _lib.TF_NO_FINAL | (_lib.TF_MOMENTS_GLOBAL if global_xy else 0) | (_lib.TF_MOMENTS_ALL if every_ray else 0)
-    with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        rc = getattr(lib, f"olb_trace_moments_{sfx}")(
-            C.byref(dtab.c), 0, dtab.table.num_surfaces if last is None else last, C.byref(la) if la is not None else None,
-            C.byref(c_rays), None, n, flags, cen, C.c_void_p(moments.data_ptr()), _ptr(status), C.c_void_p(stream))
-    _lib.check(rc, f"olb_trace_moments_{sfx}")
-    if own_status:
-        _raise_status(status)
+    _trace(dtab, dev, dtype, 0, dtab.table.num_surfaces if last is None else last, n, flags, rays=c_rays, launch=la,
+           center=center, moments=moments, status=status, own_status=status is None)
     return moments
 
 
@@ -554,7 +516,9 @@ def trace_host(dtab: DeviceTable, h_in: dict, h_out: dict, n: int, dtype=torch.f
                scratch: torch.Tensor | None = None, rec=None, first: int = 0, last: int | None = None,
                affine: dict | None = None):
     """olb_trace_host_*: HOST SoA in (pinned tensors x,y,z,L,M,N,i[,w]) -> HOST final state out
-    (x,y,z,L,M,N,i,opd); chunks are pipelined H2D / kernel / D2H on two streams."""
+    (x,y,z,L,M,N,i,opd); chunks are pipelined H2D / kernel / D2H on three streams.  With ``affine`` the host
+    pupil arrays h_in["Px"], h_in["Py"] go in instead (8 B/ray over PCIe) and the launch state is generated on
+    the device."""
     lib = dtab.lib
     sfx = _DTYPES[dtype]
     es = 4 if dtype == torch.float32 else 8
@@ -564,31 +528,19 @@ def trace_host(dtab: DeviceTable, h_in: dict, h_out: dict, n: int, dtype=torch.f
     if scratch is None or scratch.numel() < need:
         scratch = torch.empty(need, dtype=torch.uint8, device=dtab.device)
     c_out = _lib.OlbRays(**{k: h_out[k].data_ptr() for k in ("x", "y", "z", "L", "M", "N", "i", "opd")})
-    if affine is not None and dtab.table.n_wl > 1:
-        # (pupil launch: the per-ray wavelengths travel in h_out.w -- include/olb.h, olb_trace_host_pupil_*)
-        c_out.w = (h_in["w"] if "w" in h_in else h_out["w"]).data_ptr()
+    la, c_in = None, None
     if affine is not None:
-        # HOST pupil arrays in (8 B/ray over PCIe), launch state generated on the device
         la = _c_launch(affine, h_in["Px"], h_in["Py"])
-        c_rec = None
-        if rec is not None:
-            c_rec = _lib.OlbRecords(*[rec[j].data_ptr() for j in range(8)], rec.shape[-1])
-        with torch.cuda.device(dtab.device):
-            rc = getattr(lib, f"olb_trace_host_pupil_{sfx}")(
-                C.byref(dtab.c), first, last, C.byref(la), C.byref(c_out),
-                C.byref(c_rec) if c_rec is not None else None, n, chunk, C.c_void_p(scratch.data_ptr()),
-                scratch.numel(), 0, None)
-        _lib.check(rc, f"olb_trace_host_pupil_{sfx}")
-        return scratch
-    c_in = _lib.OlbRays(**{k: h_in[k].data_ptr() for k in ("x", "y", "z", "L", "M", "N", "i")},
-                        w=h_in["w"].data_ptr() if "w" in h_in and dtab.table.n_wl > 1 else None)
-    c_rec = None
-    if rec is not None:
-        c_rec = _lib.OlbRecords(*[rec[j].data_ptr() for j in range(8)], rec.shape[-1])
+        if dtab.table.n_wl > 1:
+            # (pupil launch: the per-ray wavelengths travel in h_out.w -- include/olb.h, olb_trace_host_*)
+            c_out.w = (h_in["w"] if "w" in h_in else h_out["w"]).data_ptr()
+    else:
+        c_in = _lib.OlbRays(**{k: h_in[k].data_ptr() for k in ("x", "y", "z", "L", "M", "N", "i")},
+                            w=h_in["w"].data_ptr() if "w" in h_in and dtab.table.n_wl > 1 else None)
+    c_rec = _c_records(rec) if rec is not None else None
     with torch.cuda.device(dtab.device):
         rc = getattr(lib, f"olb_trace_host_{sfx}")(
-            C.byref(dtab.c), first, last, C.byref(c_in), C.byref(c_out),
-            C.byref(c_rec) if c_rec is not None else None, n, chunk, C.c_void_p(scratch.data_ptr()),
-            scratch.numel(), 0, None)
+            C.byref(dtab.c), first, last, _byref(la), _byref(c_in), C.byref(c_out), _byref(c_rec), n, chunk,
+            C.c_void_p(scratch.data_ptr()), scratch.numel(), 0, None)
     _lib.check(rc, f"olb_trace_host_{sfx}")
     return scratch

@@ -2,7 +2,7 @@
 tolerancing Monte-Carlo shape (optiland/tolerancing/monte_carlo.py: one small trace per sampled system).
 
 Arms, all on one GPU, CUDA-event timed:
-  batch_records   one olb_trace_batch launch, shared launch rays, all record rows written
+  batch_records   one batched-table launch, shared launch rays, all record rows written
   batch_moments   one launch, shared launch rays, per-system spot moments only (no per-ray output)
   loop_single     B olb_trace launches on B pre-uploaded single-system tables (what a caller could do
                   without the batch entry point; table preparation NOT timed, so this is its best case)

@@ -120,12 +120,13 @@ def c5_call_shape_case(n):
         la = _c_launch(aff, a["Px"], a["Py"])
         c_pol = _c_polarization(None, inten)
         rays = _lib.OlbRays(w=w.data_ptr())
-        fn = getattr(dtab.lib, "olb_trace_polarized_" + tag)
+        call = _lib.OlbTraceCall(first=0, last=S, n_rays=n, flags=_lib.TF_NO_FINAL | _lib.TF_POLARIZED,
+                                 rays=C.pointer(rays), rec=C.pointer(c_rec), launch=C.pointer(la), pol=C.pointer(c_pol))
+        fn = getattr(dtab.lib, "olb_trace_call_" + tag)
         stream = torch.cuda.current_stream().cuda_stream
 
         def lean():
-            rc = fn(C.byref(dtab.c), 0, S, C.byref(la), C.byref(rays), C.byref(c_rec), n, _lib.TF_NO_FINAL, C.byref(c_pol),
-                    None, None, None, C.c_void_p(stream))
+            rc = fn(C.byref(dtab.c), C.byref(call), C.c_void_p(stream))
             assert rc == 0, _lib.last_error()
 
         ms_lean = timeit(lean)
@@ -149,7 +150,7 @@ CASES = {
     "c5shape": lambda: c5_call_shape_case(4_000_000),
     "c3grad": lambda: autograd_case(4_000_000),
     "zerngrad": lambda: autograd_case(4_000_000, "zernike_fringe", "Zernike freeform singlet: forward + backward incl. d/d Zernike "
-                                      "coefficients (olb_trace_bwd_tables_*)"),
+                                      "coefficients (olb_trace_bwd_* with grad_tables)"),
 }
 
 if __name__ == "__main__":

@@ -1,6 +1,6 @@
 """Wavefront data (OPD map + exit-pupil intercepts) for one field of the Double-Gauss, 10 M pupil samples:
-  fused      olb_trace_wavefront_*: launch generation + trace + reference-sphere epilogue, 5 values/ray written
-  unfused    olb_trace_pupil_* with full records (what Optic.trace does) + the reference's steps 4-5
+  fused      OlbTraceCall.wavefront_*: launch generation + trace + reference-sphere epilogue, 5 values/ray written
+  unfused    OlbTraceCall.launch with full records (what Optic.trace does) + the reference's steps 4-5
              (wavefront/strategy.py:179-190) as eager torch ops on the device.
 CUDA-event timed; both produce the same numbers (checked)."""
 import json

@@ -69,7 +69,7 @@ def main():
                 res[name]["p"] = float(np.max(np.abs(rays.p.cpu().numpy().astype(np.complex128) - c.out["p"])))
         path = args.gpu
         os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
-        json.dump({"cases": res, "sources": [f"{torch.cuda.get_device_name()} kernel (olb_trace_f32)"]}, open(path, "w"),
+        json.dump({"cases": res, "sources": [f"{torch.cuda.get_device_name()} kernel (olb_trace_call_f32)"]}, open(path, "w"),
                   indent=1, sort_keys=True)
         print("wrote", path)
     else:

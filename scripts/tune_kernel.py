@@ -1,4 +1,4 @@
-"""Time the device-resident trace step (one kernel launch) for the current OLB_LIB / env knobs."""
+"""Time the device-resident trace step (one kernel launch), with and without records."""
 import json
 import os
 import sys
@@ -22,8 +22,7 @@ def main():
     dev = torch.device("cuda:0")
     dtab = DeviceTable(c.table, dev)
     S = c.table.num_surfaces
-    out = {"lib": os.environ.get("OLB_LIB", "default"), "rpt": os.environ.get("OLB_FORCE_RPT", ""),
-           "grid_mult": os.environ.get("OLB_GRID_MULT", ""), "case": case, "n": n}
+    out = {"case": case, "n": n}
     for dtype, tag, es in ((torch.float32, "f32", 4), (torch.float64, "f64", 8)):
         if case == "dgauss_c2":
             g = torch.Generator(device=dev).manual_seed(0)

@@ -35,6 +35,7 @@ def test_struct_sizes_match_header():
     assert C.sizeof(_lib.OlbRecords) == 9 * 8
     assert C.sizeof(_lib.OlbTable) == 40
     assert C.sizeof(_lib.OlbDeviceTable) == 72
+    assert C.sizeof(_lib.OlbTraceCall) == 112
 
 
 def test_table_validation_errors_no_gpu_needed():

@@ -130,7 +130,7 @@ def test_config5_opd_maps_oracle_vs_reference():
 
 @pytest.mark.gpu
 def test_config5_opd_maps_kernel_within_1e5_waves():
-    """BASELINE.json config 5's tolerance, map by map, 5 fields x 3 wavelengths, through olb_trace_polarized_f64 (pupil
+    """BASELINE.json config 5's tolerance, map by map, 5 fields x 3 wavelengths, through olb_trace_call_f64, polarized (pupil
     launch + P matrices in shared memory + wavefront epilogue)."""
     import torch
 
@@ -184,7 +184,7 @@ def test_config5_generic_polarized_pupil_launch(dtype_name):
 @pytest.mark.parametrize("name", ["zernike_polarized_c5", "cooke_polarized", "tilted_fold_polarized"])
 @pytest.mark.parametrize("dtype_name", ["float64", "float32"])
 def test_intensity_epilogue_in_kernel(name, dtype_name):
-    """PolarizedRays.update_intensity as the kernel's epilogue (olb_trace_polarized_*): rays.i against the reference's
+    """PolarizedRays.update_intensity as the kernel's epilogue (OlbTraceCall.pol): rays.i against the reference's
     value; the record rows keep the geometric intensity."""
     import torch
 

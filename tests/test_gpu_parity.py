@@ -195,7 +195,7 @@ def test_host_buffer_path_matches_device_path():
 
 @pytest.mark.parametrize("name", ["generic_dgauss", "generic_litho"])
 def test_host_buffer_pupil_launch_with_per_ray_fields(name):
-    """olb_trace_host_pupil_* with launch.Hx / Hy (trace_generic's call shape from HOST arrays: pupil and field
+    """olb_trace_host_* with launch.Hx / Hy (trace_generic's call shape from HOST arrays: pupil and field
     coordinates + wavelengths cross PCIe, the launch state is generated on the device) == the device-resident launch,
     bit for bit, and the reference's records within tolerance."""
     from optiland_b200.launch import pupil_affine_fields
@@ -390,7 +390,7 @@ def test_autograd_ray_input_gradients_and_unsupported_tables():
 
 @pytest.mark.parametrize("name", ["zernike_fringe", "zernike_standard", "misc_apertures_coatings", "chebyshev"])
 def test_polynomial_family_adjoint_kernel(name):
-    """olb_trace_bwd_tables_* on the GPU (Zernike / polynomial / Chebyshev surfaces): gradients of a random linear functional of all
+    """olb_trace_bwd_* with grad_tables on the GPU (Zernike / polynomial / Chebyshev surfaces): gradients of a random linear functional of all
     records w.r.t. the launch state, the surface parameters and the USER coefficients (table gradients mapped back)
     against the CPU instantiation of the same adjoint, which tests/test_hostcheck_backward.py holds to finite differences
     of the oracle; fp32 against fp64."""
@@ -579,8 +579,9 @@ def test_per_ray_field_launch_matches_reference_trace_generic(name, dtype):
         assert max_abs_err(_np(rec[k]), c.rec[k]) <= (tol if k not in ("L", "M", "N") or f64 else 5e-6), k
 
 
-def test_c_abi_error_codes_on_device_calls():
-    """Bad arguments are reported through return codes + olb_last_error, never by crashing."""
+def test_c_abi_error_codes_on_trace_call_entry_points():
+    """Bad arguments to olb_trace_call_* / olb_trace_bwd_* are reported through return codes + olb_last_error, never by
+    crashing."""
     import ctypes as C
 
     from optiland_b200 import _lib
@@ -595,9 +596,12 @@ def test_c_abi_error_codes_on_device_calls():
     good = dict(zip(("x", "y", "z", "L", "M", "N", "i", "opd"), ptrs))
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
+    def trace(table, **fields):
+        return lib.olb_trace_call_f32(C.byref(table.c), C.byref(_lib.OlbTraceCall(**fields)), stream)
+
     def call(rays, first=0, last=13, rec=None, flags=0, nn=n):
-        return lib.olb_trace_f32(C.byref(dt.c), first, last, C.byref(rays), C.byref(rec) if rec else None, nn, flags,
-                                 None, stream)
+        return trace(dt, first=first, last=last, n_rays=nn, flags=flags, rays=C.pointer(rays),
+                     rec=C.pointer(rec) if rec else None)
 
     assert call(_lib.OlbRays(**good)) == 0
     bad = dict(good); bad["z"] = None
@@ -611,7 +615,8 @@ def test_c_abi_error_codes_on_device_calls():
     assert call(_lib.OlbRays(**good), rec=rec) == -1 and "row_stride" in _lib.last_error()
     assert call(_lib.OlbRays(**good), nn=0) == 0          # empty batch: nothing to do
     fake = _lib.OlbDeviceTable()
-    assert lib.olb_trace_f32(C.byref(fake), 0, 1, C.byref(_lib.OlbRays(**good)), None, n, 0, None, stream) == -1
+    assert lib.olb_trace_call_f32(C.byref(fake), C.byref(_lib.OlbTraceCall(last=1, n_rays=n, rays=C.pointer(
+        _lib.OlbRays(**good)))), stream) == -1
     # wavefront epilogue: argument validation
     from optiland_b200.launch import pupil_affine
     from optiland_b200.trace import _c_launch
@@ -624,9 +629,9 @@ def test_c_abi_error_codes_on_device_calls():
     ref.radius, ref.n_image, ref.wavelength_um = 100.0, 1.0, 0.55
 
     def wf(ref_, out_, launch=la, last=13):
-        return lib.olb_trace_wavefront_f32(C.byref(dt.c), 0, last, C.byref(launch) if launch is not None else None,
-                                           C.byref(_lib.OlbRays(**good)), None, n, _lib.TF_NO_FINAL, C.byref(ref_),
-                                           C.byref(out_), None, stream)
+        return trace(dt, last=last, n_rays=n, flags=_lib.TF_NO_FINAL, rays=C.pointer(_lib.OlbRays(**good)),
+                     launch=C.pointer(launch) if launch is not None else None, wavefront_ref=C.pointer(ref_),
+                     wavefront_out=C.pointer(out_))
 
     assert wf(ref, out) == 0
     assert wf(ref, out, last=12) == -1 and "image surface" in _lib.last_error()
@@ -637,18 +642,17 @@ def test_c_abi_error_codes_on_device_calls():
     tilted.radius, tilted.n_image, tilted.wavelength_um = 100.0, 1.0, 0.55
     tilted.tilt = (C.c_double * 2)(0.0, 1.5)
     assert wf(tilted, out, launch=None) == -1 and "pupil samples" in _lib.last_error()
-    # batched tables: wrong entry point / ray count
+    # batched tables: rays_per_system missing / ray count
     from optiland_b200.batch import BatchedTable, template_params
 
     bt = BatchedTable(c.table, np.repeat(template_params(c.table)[None], 3, axis=0))
-    assert lib.olb_trace_f32(C.byref(bt.c), 0, 13, C.byref(_lib.OlbRays(**good)), None, n, 0, None, stream) == -1
+    good_rays = C.pointer(_lib.OlbRays(**good))
+    assert trace(bt, last=13, n_rays=n, rays=good_rays) == -1
     assert "several systems" in _lib.last_error()
-    cen = (C.c_double * 2)(0.0, 0.0)
-    assert lib.olb_trace_batch_f32(C.byref(bt.c), 0, 13, C.byref(_lib.OlbRays(**good)), None, 100, 0, cen, None, None,
-                                   stream) == 0      # 3 x 100 rays of the 1024-ray buffers
-    assert lib.olb_trace_batch_f32(C.byref(bt.c), 0, 13, C.byref(_lib.OlbRays(**good)), None, 100, _lib.TF_SHARED_INPUT,
-                                   cen, None, None, stream) == -1 and "SHARED_INPUT" in _lib.last_error()
-    assert lib.olb_trace_bwd_f32(C.byref(bt.c), 0, 13, None, None, None, None, None, n, C.c_uint64(0), stream) != 0
+    assert trace(bt, last=13, n_rays=300, rays=good_rays, rays_per_system=100) == 0   # 3 x 100 rays of the 1024-ray buffers
+    assert trace(bt, last=13, n_rays=300, rays=good_rays, rays_per_system=100, flags=_lib.TF_SHARED_INPUT) == -1
+    assert "SHARED_INPUT" in _lib.last_error()
+    assert lib.olb_trace_bwd_f32(C.byref(bt.c), 0, 13, None, None, None, None, None, None, n, C.c_uint64(0), stream) != 0
     torch.cuda.synchronize()
 
 
@@ -716,7 +720,7 @@ def test_plugin_cuda_engine_on_optiland_shaped_rays():
     tr = types.SimpleNamespace(**{k: torch.from_numpy(t.rays[k]).cuda() for k in ("x", "y", "z", "L", "M", "N", "i", "w")})
     tr.opd = torch.zeros_like(tr.x)
     assert eng.trace_grad(t.table, AG.table_to_params(t.table).cuda(), tr) is not None  # tilted poses are in scope
-    z = Case("zernike_fringe")      # Zernike / polynomial surfaces: in scope since round 2 (olb_trace_bwd_tables_*)
+    z = Case("zernike_fringe")      # Zernike / polynomial surfaces: in scope since round 2 (grad_tables)
     zr = types.SimpleNamespace(**{k: torch.from_numpy(z.rays[k]).cuda() for k in ("x", "y", "z", "L", "M", "N", "i", "w")})
     zr.opd = torch.zeros_like(zr.x)
     assert eng.trace_grad(z.table, AG.table_to_params(z.table).cuda(), zr, coefs=AG.table_to_coefs(z.table).cuda()) is not None

@@ -265,7 +265,7 @@ def test_odd_asphere_adjoint_on_the_vertex_ray(hc):
 
 @pytest.mark.parametrize("name", ["zernike_fringe", "zernike_noll", "misc_apertures_coatings"])
 def test_polynomial_family_adjoint_matches_finite_differences(hc, name):
-    """The adjoint through Zernike / polynomial surfaces (olb_trace_bwd_tables_*: implicit-function theorem with the true
+    """The adjoint through Zernike / polynomial surfaces (olb_trace_bwd_* with grad_tables: implicit-function theorem with the true
     sag gradient, the Hessian of the reference's slope polynomial for the normal, table gradients mapped back to the user
     coefficients): launch-state gradients, curvature / conic / pose of the freeform surface and EVERY coefficient against
     central differences of the oracle."""

@@ -593,7 +593,7 @@ def test_autograd_tilt_and_decenter_variables_match_reference_eager_graph(plugin
 def test_autograd_zernike_and_polynomial_coefficient_variables(plugin):
     """Freeform optimisation variables through the capability: d(RMS spot)/d(Zernike coefficient), d/d(polynomial
     coefficient), d/d(Chebyshev coefficient), d/d(radius, conic) of the freeform surface -- forward kernel + the polynomial-family adjoint
-    (olb_trace_bwd_tables_*: table gradients mapped back to the live coefficient tensors) -- equal the reference's own
+    (olb_trace_bwd_* grad_tables: table gradients mapped back to the live coefficient tensors) -- equal the reference's own
     eager autograd, with the coefficients set the way ZernikeCoeffVariable / PolynomialCoeffVariable set them
     (optimization/variable/zernike_coeff.py:71-95: ``geometry.coefficients[i] = value``; polynomial_coeff.py:77-81 and its
     subclass chebyshev_coeff.py: ``geometry.coefficients[i][j] = value``)."""

@@ -18,7 +18,7 @@ from tests.test_plugin_reference import plugin  # noqa: F401  (fixture: [oracle]
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype_name", ["float64", "float32"])
 def test_forbes_adjoint_kernel_matches_cpu_instantiation(dtype_name):
-    """olb_trace_bwd_tables_* on a table with two Forbes Q^bfs surfaces (the `forbes_qbfs` fixture): gradients of a random
+    """olb_trace_bwd_* with grad_tables on a table with two Forbes Q^bfs surfaces (the `forbes_qbfs` fixture): gradients of a random
     linear functional of all records w.r.t. the launch state and every surface parameter -- the coefficient slots hold
     dLoss/db_m (Clenshaw basis), mapped to the user's a_m by ``_TraceFn.backward`` -- against the CPU instantiation of the
     same adjoint, which tests/test_hostcheck_backward.py holds to finite differences of the oracle."""
