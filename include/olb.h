@@ -38,7 +38,7 @@ extern "C" {
 #endif
 
 #define OLB_VERSION_MAJOR 0
-#define OLB_VERSION_MINOR 2
+#define OLB_VERSION_MINOR 3
 
 /* ---- error codes ------------------------------------------------------- */
 #define OLB_OK                 0
@@ -87,6 +87,29 @@ extern "C" {
 #define OLB_COAT_SIMPLE    1   /* SimpleCoating: i *= T or R (optiland/coatings.py:164-237) */
 #define OLB_COAT_FRESNEL   2   /* FresnelCoating (optiland/coatings.py:362-386,
                                   optiland/jones.py:71-117); needs polarized rays       */
+
+/* ---- interaction models (OlbSurface.interaction) ------------------------
+ * 0 is the refractive / reflective model (optiland/interactions/refractive_reflective_model.py).  The
+ * others are PhaseInteractionModel (optiland/interactions/phase_interaction_model.py:45-132), the generalized
+ * Snell's law of a phase profile phi(x, y) on the surface, in the local frame, with k0 = 2 pi / (lambda * 1e-3):
+ *     k_par = n1 k0 d - (n1 k0 d . n) n + grad phi - (grad phi . n) n,   R^2 = (n2 k0)^2 - |k_par|^2
+ *     R^2 < 0 -> i := 0 and R^2 := 0 (evanescent: no NaN);  d := normalise(k_par +- sqrt(R^2) n)
+ *     (+ refraction, - reflection; n2 := n1 for a reflective surface);  opd += -phi / k0;  i *= efficiency
+ * with the geometry's normal n AS IT RETURNS IT (no alignment with the ray: on a curved substrate, whose
+ * normal points to -z, transmitted rays leave backwards -- the reference's behaviour, reproduced).  The
+ * coating step (SimpleCoating / FresnelCoating / the polarization update) follows as for refraction.
+ * Block at pool[phase_off]: {efficiency, n_terms, params[n_terms]} with
+ *   CONSTANT : n_terms = 1, {phi}                                 (phase/constant.py)
+ *   LINEAR   : n_terms = 2, {Kx, Ky}: phi = Kx x + Ky y           (phase/linear_grating.py, its _K_x / _K_y)
+ *   RADIAL   : 1 <= n_terms <= OLB_MAX_PHASE_TERMS, {a_1 .. a_n}: phi = sum_p a_p r^(2p)  (phase/radial.py)
+ * 1 / k0 per wavelength is derived at upload from the table's wavelength list.  A table with a phase surface
+ * has bwd_supported = 0 and olb_table_upload_batch rejects it (OLB_ERR_UNSUPPORTED).
+ */
+#define OLB_INTERACT_REFRACT        0
+#define OLB_INTERACT_PHASE_CONSTANT 1
+#define OLB_INTERACT_PHASE_LINEAR   2
+#define OLB_INTERACT_PHASE_RADIAL   3
+#define OLB_MAX_PHASE_TERMS        16
 
 /* ---- aperture programs --------------------------------------------------
  * surface.aperture (optiland/physical_apertures/*.py) is flattened by the host
@@ -152,7 +175,8 @@ typedef struct OlbSurface {
   int32_t coating;     /* OLB_COAT_*                                          */
   int32_t media_off;   /* pool offset of the 5 x n_wl media block             */
   int32_t aux0;        /* polynomial: number of columns (y powers)            */
-  int32_t reserved[2];
+  int32_t interaction; /* OLB_INTERACT_* (0: refractive / reflective)          */
+  int32_t phase_off;   /* pool offset of the phase-profile block (see above)  */
   double t[3];         /* effective translation                               */
   double R[9];         /* effective rotation, row-major                       */
   double radius;       /* geometry.radius (inf => plane branch of Standard)   */

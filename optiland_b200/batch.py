@@ -28,6 +28,8 @@ def template_params(table: T.SurfaceTable) -> np.ndarray:
     """(S, BP_COUNT) block of the template's own values."""
     if table.n_wl != 1:
         raise ValueError("batched tables support one wavelength")
+    if any(s.interaction != T.INTERACT_REFRACT for s in table.surfaces):
+        raise ValueError("batched tables with phase-profile surfaces are not built")
     p = np.zeros((table.num_surfaces, _lib.BP_COUNT))
     for s, spec in enumerate(table.surfaces):
         p[s, _lib.BP_TX:_lib.BP_TX + 3] = spec.t

@@ -913,6 +913,61 @@ OLB_HD T polarized_intensity(const T* P, int ps, T kx, T ky, T kz, T i0, int mod
   return total * i0 / (T)n_states;
 }
 
+// Phase-profile interaction (PhaseInteractionModel.interact_real_rays, phase_interaction_model.py:45-124): the
+// generalized Snell's law with the geometry's UNALIGNED normal n (include/olb.h, OLB_INTERACT_*).  The wave vectors
+// are carried in units of k0 (k / k0, grad phi / k0), which leaves the direction unchanged and keeps every term O(1)
+// in fp32.  `n1` is material_pre's index (NaN for an unknown wavelength).  Efficiency is applied by the caller after
+// the coating step, as in the reference.
+template <typename T>
+OLB_HD void phase_interact(Ray<T>& r, const PrepSurface<T>& S, const T* pool, T nx, T ny, T nz, T n1) {
+  const T* ph = pool + S.phase_off;
+  const int nt = (int)ph[PH_NT];
+  const T* c = ph + PH_P;
+  const T* wl = c + (S.phase == OLB_INTERACT_PHASE_RADIAL ? 2 * nt : nt) + 2 * (r.widx < 0 ? 0 : r.widx);
+  const T ik0 = wl[0], n2 = wl[1] + (n1 - n1);   // (n1 - n1: NaN for an unknown wavelength, 0 otherwise)
+  T phi, gx, gy;
+  if (S.phase == OLB_INTERACT_PHASE_RADIAL) {
+    // phi = sum a_p r^(2p), grad phi = (x, y) sum 2p a_p r^(2p-2): Horner in r^2, no division (0 on axis)
+    const T r2 = o_fma(r.x, r.x, r.y * r.y);
+    T v = 0, d = 0;
+    for (int p = nt - 1; p >= 0; --p) {
+      v = o_fma(v, r2, c[p]);
+      d = o_fma(d, r2, c[nt + p]);
+    }
+    phi = v * r2;
+    gx = d * r.x;
+    gy = d * r.y;
+  } else if (S.phase == OLB_INTERACT_PHASE_LINEAR) {
+    phi = o_fma(c[0], r.x, c[1] * r.y);
+    gx = c[0];
+    gy = c[1];
+  } else {
+    phi = c[0];
+    gx = 0;
+    gy = 0;
+  }
+  // G = grad phi - (grad phi . n) n ;  k_par = k_in - (k_in . n) n + G  (grad phi has no z component)
+  gx *= ik0; gy *= ik0;
+  const T gdn = o_fma(gx, nx, gy * ny);
+  const T ax = n1 * r.L, ay = n1 * r.M, az = n1 * r.N;
+  const T kdn = o_fma(ax, nx, o_fma(ay, ny, az * nz));
+  const T px = o_fma(-kdn, nx, ax) + o_fma(-gdn, nx, gx);
+  const T py = o_fma(-kdn, ny, ay) + o_fma(-gdn, ny, gy);
+  const T pz = o_fma(-kdn, nz, az) - gdn * nz;
+  T R2 = o_fma(n2, n2, -o_fma(px, px, o_fma(py, py, pz * pz)));
+  if (R2 < 0) {           // evanescent: clipped, and a finite grazing direction (R^2 := 0; NaN stays NaN)
+    r.i = 0;
+    R2 = 0;
+  }
+  const T al = (S.flags & OLB_SF_REFLECT) ? -o_sqrt(R2) : o_sqrt(R2);
+  const T kx = o_fma(al, nx, px), ky = o_fma(al, ny, py), kz = o_fma(al, nz, pz);
+  const T inv = o_rsqrt(o_fma(kx, kx, o_fma(ky, ky, kz * kz)));
+  r.L = kx * inv;
+  r.M = ky * inv;
+  r.N = kz * inv;
+  accumulate_opd(r, -phi * ik0);   // opd += -phi / k0 (signed)
+}
+
 // The surface step.  FEAT gates code that most systems never need (register pressure, code
 // size); KIND (0 plane, 1 sphere/conic closed form, 2 Newton family) is resolved by the caller
 // ONCE per surface, outside the per-ray loop, so the hot loop carries no geometry branches.
@@ -986,8 +1041,17 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
 
   // -- interaction (refractive_reflective_model.py:32-55)
   if (FEAT & (FEAT_EXTRA | FEAT_POL)) { r.L0 = r.L; r.M0 = r.M; r.N0 = r.N; }
+  bool phase = false;
+  if constexpr ((FEAT & FEAT_PHASE) != 0) {
+    // phase-profile surface (phase_interaction_model.py:45-132): replaces refract / reflect
+    if (S.phase != OLB_INTERACT_REFRACT) {
+      phase_interact(r, S, pool, nx, ny, nz, med[MED_N1] + bad);
+      phase = true;
+    }
+  }
   T dot = o_fma(r.L, nx, o_fma(r.M, ny, r.N * nz));
-  if (S.flags & OLB_SF_REFLECT) {
+  if (phase) {
+  } else if (S.flags & OLB_SF_REFLECT) {
     // real_rays.py:189-205 with the aligned normal: d - 2 |dot| sign(dot) n = d - 2 dot n
     T m2 = -2 * dot;
     r.L = o_fma(m2, nx, r.L);
@@ -1019,6 +1083,10 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
       // (Pm is the caller's matrix storage -- never a pointer into `r`: taking r.P's address here would force the
       // whole ray state into local memory in the kernel)
       polar_update(r, Pm, Pstride, S, med[MED_CN] + bad, o_abs(o_fma(r.L0, nx, o_fma(r.M0, ny, r.N0 * nz))));
+  }
+  // -- phase profile efficiency (phase_interaction_model.py:129-130)
+  if constexpr ((FEAT & FEAT_PHASE) != 0) {
+    if (phase) r.i *= pool[S.phase_off + PH_EFF];
   }
 }
 

@@ -32,7 +32,15 @@ enum : uint32_t {
   FEAT_EXTRA = 1u << 2,    // non-radial aperture programs, simple coatings, L0/M0/N0 output
   FEAT_POL = 1u << 3,      // polarized rays (P matrix) / Fresnel coatings
   FEAT_FREEFORM = 1u << 4, // polynomial / Zernike / Chebyshev / biconic / toroidal / Forbes surfaces (with NEWTON)
+  FEAT_PHASE = 1u << 5,    // a phase-profile surface (PhaseInteractionModel): runs the general kernel + this
 };
+
+// Prepared phase block per surface (PrepSurface::phase_off), elements of T:
+//   [PH_EFF] efficiency, [PH_NT] number of profile terms n, then from PH_P the profile terms:
+//   constant {phi}; linear {Kx, Ky}; radial {a_1 .. a_n, 2 a_1, 4 a_2 .. 2n a_n} (value and gradient Horner
+//   coefficients in r^2); then, per wavelength j, {1 / k0 = lambda_j * 1e-3 / (2 pi) (mm / rad), n2 of the
+//   interaction (n1 when reflective, phase_interaction_model.py:53-56)}.
+enum { PH_EFF = 0, PH_NT = 1, PH_P = 2 };
 
 struct PrepHeader {
   int32_t n_surf;
@@ -67,7 +75,9 @@ struct PrepSurface {
   int32_t poly_d_off;  // pool offset of the derivative-source table (Zernike quirk)
   int32_t gslot;       // backward: first per-thread gradient accumulator slot of this surface
   int32_t gslots;      //           number of slots (7 + n_coef [+ 9 for a tilted pose]; 0 for NOOP)
-  int32_t pad16[2];    // keeps sizeof a multiple of 16 (256 / 448 bytes): the pool behind the array stays 16-byte aligned
+  int32_t phase;       // OLB_INTERACT_* (0: refractive / reflective); read by FEAT_PHASE kernels only
+  int32_t phase_off;   // pool offset of the prepared phase block (PH_* below)
+  // (sizeof stays a multiple of 16 (256 / 448 bytes): the pool behind the array stays 16-byte aligned)
   // incoming transform from GLOBAL coordinates: p_loc = Ag * p + bg
   T Ag[9], bg[3];
   // incoming transform from the PREVIOUS surface's local frame: p_loc = Ar * p + br
@@ -173,6 +183,7 @@ static void build_blob(const OlbTable& tab, const std::vector<std::vector<double
     b.max_iter = a.max_iter; b.coating = a.coating; b.media_off = a.media_off + base;
     b.poly_rows = a.poly_rows; b.poly_cols = a.poly_cols; b.poly_d_off = a.poly_d_off + base;
     b.gslot = a.gslot; b.gslots = a.gslots;
+    b.phase = a.phase; b.phase_off = a.phase ? a.phase_off + base : 0;
     for (int i = 0; i < 9; ++i) { b.Ag[i] = (T)a.Ag[i]; b.Ar[i] = (T)a.Ar[i]; b.R[i] = (T)a.R[i]; }
     for (int i = 0; i < 3; ++i) { b.bg[i] = (T)a.bg[i]; b.br[i] = (T)a.br[i]; b.t[i] = (T)a.t[i]; }
     b.radius = (T)a.radius; b.curv = (T)a.curv; b.conic = (T)a.conic; b.kp1 = (T)a.kp1;
@@ -468,6 +479,38 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     if (in.coating == OLB_COAT_SIMPLE) features |= FEAT_EXTRA;
     else if (in.coating == OLB_COAT_FRESNEL) features |= FEAT_POL;
     else if (in.coating != OLB_COAT_NONE) { res.error = "unknown coating"; return res; }
+
+    // ---- phase-profile interaction (PhaseInteractionModel) ---------------------------------------
+    if (in.interaction != OLB_INTERACT_REFRACT) {
+      if (in.interaction < OLB_INTERACT_PHASE_CONSTANT || in.interaction > OLB_INTERACT_PHASE_RADIAL) {
+        res.error = "unknown interaction model"; return res;
+      }
+      if (in.kind == OLB_GEOM_NOOP) { res.error = "phase interaction on an object surface"; return res; }
+      if (!in_pool(in.phase_off, 2)) { res.error = "phase block outside pool"; return res; }
+      const double eff = tab.pool[in.phase_off], ntd = tab.pool[in.phase_off + 1];
+      const int nt = (int)ntd;
+      const int want = in.interaction == OLB_INTERACT_PHASE_CONSTANT ? 1 : in.interaction == OLB_INTERACT_PHASE_LINEAR ? 2 : -1;
+      if (!(ntd == (double)nt) || (want > 0 && nt != want) || (want < 0 && (nt < 1 || nt > OLB_MAX_PHASE_TERMS))) {
+        res.error = "bad phase block: wrong number of profile terms"; return res;
+      }
+      if (!in_pool(in.phase_off, 2 + nt)) { res.error = "phase block outside pool"; return res; }
+      if (!std::isfinite(eff)) { res.error = "bad phase block: non-finite efficiency"; return res; }
+      const double* prm = tab.pool + in.phase_off + 2;
+      o.phase = in.interaction;
+      o.phase_off = (int)pool.size();
+      pool.push_back(eff);
+      pool.push_back((double)nt);
+      for (int p = 0; p < nt; ++p) pool.push_back(prm[p]);
+      if (in.interaction == OLB_INTERACT_PHASE_RADIAL)
+        for (int p = 0; p < nt; ++p) pool.push_back(2.0 * (p + 1) * prm[p]);
+      for (int j = 0; j < n_wl; ++j) {
+        pool.push_back(tab.wavelengths[j] * 1e-3 / (2.0 * M_PI));
+        pool.push_back((in.flags & OLB_SF_REFLECT) ? tab.pool[in.media_off + j] : tab.pool[in.media_off + n_wl + j]);
+      }
+      while (pool.size() % 4) pool.push_back(0);
+      features |= FEAT_PHASE;
+      res.bwd_supported = false;       // the adjoint has no phase interaction
+    }
   }
   res.features = features;
   int gslot = 0;
@@ -515,6 +558,10 @@ static BatchPrep prepare_batch(const OlbTable& tmpl, const double* params, int n
   BatchPrep out;
   if (tmpl.n_wl != 1) { out.error = "batched tables support one wavelength"; out.unsupported = true; return out; }
   const int S = tmpl.n_surfaces;
+  for (int s = 0; s < S && tmpl.surfaces; ++s)
+    if (tmpl.surfaces[s].interaction != OLB_INTERACT_REFRACT) {
+      out.error = "batched tables with phase-profile surfaces are not built"; out.unsupported = true; return out;
+    }
   std::vector<OlbSurface> surf(tmpl.surfaces, tmpl.surfaces + S);
   std::vector<double> pool(tmpl.pool, tmpl.pool + tmpl.pool_len);
   OlbTable t = tmpl;

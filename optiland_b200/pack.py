@@ -105,6 +105,10 @@ class _Prefetch:
             z = getattr(g, "zernike", None)
             if z is not None:
                 self._add(list(getattr(z, "coeffs", [])))
+            pp = getattr(getattr(surf, "interaction_model", None), "phase_profile", None)
+            if pp is not None:      # phase-profile terms (pack_phase_profile)
+                for k in ("phase", "_K_x", "_K_y", "coefficients"):
+                    self._add(getattr(pp, k, None))
             ap = getattr(surf, "aperture", None)
             stack = [ap] if ap is not None else []
             while stack:
@@ -251,6 +255,27 @@ _GEOM_KINDS = {
 }
 
 
+def pack_phase_profile(profile) -> tuple[int, np.ndarray, float]:
+    """(interaction kind, terms, efficiency) of a ``PhaseInteractionModel``'s profile (optiland/phase/*.py).  Only the
+    exact profile classes are accepted: a subclass may override get_phase / get_gradient."""
+    name = _cls(profile)
+    if name == "ConstantPhaseProfile":
+        kind, terms = T.INTERACT_PHASE_CONSTANT, [_f(profile.phase)]
+    elif name == "LinearGratingPhaseProfile":
+        # the profile's own precomputed K_x / K_y (linear_grating.py:51-54), so the rounding matches
+        kind, terms = T.INTERACT_PHASE_LINEAR, [_f(profile._K_x), _f(profile._K_y)]
+    elif name == "RadialPhaseProfile":
+        coefs = list(profile.coefficients)
+        if not coefs:
+            raise UnsupportedSurface("RadialPhaseProfile without coefficients")
+        if len(coefs) > T.MAX_PHASE_TERMS:
+            raise UnsupportedSurface(f"RadialPhaseProfile with more than {T.MAX_PHASE_TERMS} coefficients")
+        kind, terms = T.INTERACT_PHASE_RADIAL, [_f(c) for c in coefs]
+    else:
+        raise UnsupportedSurface(f"phase profile {name}")
+    return kind, np.array(terms, dtype=np.float64), _f(profile.efficiency)
+
+
 def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     """One Optiland ``Surface`` / ``ObjectSurface`` / ``ImageSurface`` -> ``SurfaceSpec``."""
     sname = _cls(surface)
@@ -268,16 +293,20 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     kind = _GEOM_KINDS[gname]
 
     im = surface.interaction_model
-    if _cls(im) != "RefractiveReflectiveModel":
-        raise UnsupportedSurface(f"interaction model {_cls(im)}")
+    iname = _cls(im)
+    if iname not in ("RefractiveReflectiveModel", "PhaseInteractionModel"):
+        raise UnsupportedSurface(f"interaction model {iname}")
     if getattr(im, "bsdf", None) is not None:
         raise UnsupportedSurface("bsdf scatter")
+    phase = pack_phase_profile(im.phase_profile) if iname == "PhaseInteractionModel" else None
 
     t_eff, R_eff = _pose(g.cs)
     if not (np.all(np.isfinite(t_eff)) and np.all(np.isfinite(R_eff))):
         raise UnsupportedSurface("non-finite pose")
 
     spec = T.SurfaceSpec(kind=kind, t=t_eff, R=R_eff, reflective=bool(im.is_reflective))
+    if phase is not None:
+        spec.interaction, spec.phase_terms, spec.phase_efficiency = phase
     if kind != T.GEOM_PLANE:
         spec.radius = _f(g.radius)
         spec.conic = _f(g.k)

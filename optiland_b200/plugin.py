@@ -592,6 +592,8 @@ def _live_params(surfaces, table, wavelength):
     flat, flat_r = [], []
     for surf, spec in zip(surfaces, table.surfaces):
         vals = [zero] * GP_COUNT
+        if spec.interaction != T.INTERACT_REFRACT:
+            return None          # phase-profile surfaces: the adjoint has no phase interaction
         if spec.kind != T.GEOM_NOOP:
             g = surf.geometry
             cs = g.cs
@@ -732,6 +734,12 @@ def _wants_grad(backend, surfaces, rays=None) -> bool:
         coefs = getattr(g, "coefficients", None)     # (Zernike: the property returns geometry.zernike.coeffs)
         if coefs is not None:
             vals += [coefs] if hasattr(coefs, "requires_grad") else list(np.ravel(np.asarray(coefs, dtype=object)))
+        pp = getattr(getattr(surf, "interaction_model", None), "phase_profile", None)
+        if pp is not None:                           # phase-profile terms (pack.pack_phase_profile)
+            vals += [getattr(pp, k, None) for k in ("phase", "_K_x", "_K_y")]
+            pc = getattr(pp, "coefficients", None)
+            if pc is not None:
+                vals += [pc] if hasattr(pc, "requires_grad") else list(np.ravel(np.asarray(pc, dtype=object)))
         if any(rg(v) for v in vals):
             return True
     return False

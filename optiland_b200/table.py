@@ -41,6 +41,13 @@ COAT_NONE = 0
 COAT_SIMPLE = 1
 COAT_FRESNEL = 2
 
+INTERACT_REFRACT = 0
+INTERACT_PHASE_CONSTANT = 1
+INTERACT_PHASE_LINEAR = 2
+INTERACT_PHASE_RADIAL = 3
+MAX_PHASE_TERMS = 16
+_PHASE_TERMS = {INTERACT_PHASE_CONSTANT: 1, INTERACT_PHASE_LINEAR: 2}
+
 AP_RADIAL = 1
 AP_OFFSET_RADIAL = 2
 AP_RECT = 3
@@ -67,7 +74,7 @@ OLB_SURFACE_DTYPE = np.dtype(
     [
         ("kind", "<i4"), ("flags", "<u4"), ("n_coef", "<i4"), ("coef_off", "<i4"),
         ("aper_off", "<i4"), ("aper_len", "<i4"), ("max_iter", "<i4"), ("coating", "<i4"),
-        ("media_off", "<i4"), ("aux0", "<i4"), ("reserved", "<i4", (2,)),
+        ("media_off", "<i4"), ("aux0", "<i4"), ("interaction", "<i4"), ("phase_off", "<i4"),
         ("t", "<f8", (3,)), ("R", "<f8", (9,)),
         ("radius", "<f8"), ("conic", "<f8"), ("tol", "<f8"),
         ("coat_t", "<f8"), ("coat_r", "<f8"), ("norm_radius", "<f8"),
@@ -108,6 +115,12 @@ class SurfaceSpec:
     # ZERNIKE only, host side only (not packed): the normalisation constants N_nm per term, for mapping table
     # gradients back to the coefficients when a coefficient is exactly 0 (c * N_nm then does not reveal N_nm)
     zernike_norms: np.ndarray | None = None
+    # phase-profile interaction (PhaseInteractionModel, include/olb.h OLB_INTERACT_*): INTERACT_REFRACT for the
+    # refractive / reflective model; otherwise the profile's terms (constant {phi}, linear {Kx, Ky}, radial
+    # {a_1 .. a_n}) and its diffraction efficiency
+    interaction: int = INTERACT_REFRACT
+    phase_terms: np.ndarray = field(default_factory=lambda: np.zeros(0))
+    phase_efficiency: float = 1.0
 
     def __post_init__(self):
         self.t = np.asarray(self.t, dtype=np.float64).reshape(3)
@@ -116,6 +129,7 @@ class SurfaceSpec:
         self.n1 = np.atleast_1d(np.asarray(self.n1, dtype=np.float64))
         self.n2 = np.atleast_1d(np.asarray(self.n2, dtype=np.float64))
         self.k1 = np.atleast_1d(np.asarray(self.k1, dtype=np.float64))
+        self.phase_terms = np.atleast_1d(np.asarray(self.phase_terms, dtype=np.float64)).ravel()
         if self.aperture is not None:
             self.aperture = np.asarray(self.aperture, dtype=np.float64).ravel()
         if self.coat_n1 is not None:
@@ -191,6 +205,12 @@ class SurfaceTable:
                 validate_aperture_program(s.aperture)
             if s.coating == COAT_FRESNEL and (s.coat_n1 is None or s.coat_n2 is None):
                 raise ValueError("Fresnel coating needs coat_n1/coat_n2")
+            if s.interaction != INTERACT_REFRACT:
+                nt = len(s.phase_terms)
+                if s.interaction not in (INTERACT_PHASE_CONSTANT, INTERACT_PHASE_LINEAR, INTERACT_PHASE_RADIAL):
+                    raise ValueError(f"unknown interaction {s.interaction}")
+                if nt != _PHASE_TERMS.get(s.interaction, nt) or not 1 <= nt <= MAX_PHASE_TERMS:
+                    raise ValueError(f"phase profile: {nt} terms for interaction {s.interaction}")
 
     @property
     def num_surfaces(self) -> int:
@@ -218,7 +238,8 @@ class SurfaceTable:
 
         # integer / offset columns are filled per surface, then every struct field is assigned ONCE for all
         # surfaces (a per-element structured assignment costs ~1 us; this runs on every plugin call)
-        ints = {k: [0] * n for k in ("n_coef", "aux0", "coef_off", "aper_off", "aper_len", "media_off")}
+        ints = {k: [0] * n for k in ("n_coef", "aux0", "coef_off", "aper_off", "aper_len", "media_off", "interaction",
+                                     "phase_off")}
         for j, s in enumerate(self.surfaces):
             coef = s.coefficients
             extra_head = None
@@ -247,6 +268,9 @@ class SurfaceTable:
             cn2 = s.coat_n2 if s.coat_n2 is not None else s.n2
             ints["media_off"][j] = push(np.concatenate([s.n1, s.n2, s.k1, cn1, cn2]))
             assert len(s.n1) == n_wl
+            if s.interaction != INTERACT_REFRACT:
+                ints["interaction"][j] = s.interaction
+                ints["phase_off"][j] = push(np.concatenate([[s.phase_efficiency, float(len(s.phase_terms))], s.phase_terms]))
         for k, v in ints.items():
             surf[k] = v
         sl = self.surfaces
@@ -330,6 +354,12 @@ class SurfaceTable:
             m0 = int(r["media_off"])
             media = pool[m0: m0 + 5 * n_wl].reshape(5, n_wl)
             coating = int(r["coating"])
+            inter = int(r["interaction"])
+            phase = {}
+            if inter != INTERACT_REFRACT:
+                p0 = int(r["phase_off"])
+                phase = dict(interaction=inter, phase_efficiency=float(pool[p0]),
+                             phase_terms=pool[p0 + 2: p0 + 2 + int(pool[p0 + 1])].copy())
             specs.append(
                 SurfaceSpec(
                     kind=kind, t=r["t"].copy(), R=r["R"].reshape(3, 3).copy(),
@@ -345,6 +375,7 @@ class SurfaceTable:
                     coat_n1=media[3].copy() if coating == COAT_FRESNEL else None,
                     coat_n2=media[4].copy() if coating == COAT_FRESNEL else None,
                     record=not (flags & SF_NORECORD),
+                    **phase,
                 )
             )
         return cls(specs, wavelengths)
