@@ -104,11 +104,35 @@ extern "C" {
  *   RADIAL   : 1 <= n_terms <= OLB_MAX_PHASE_TERMS, {a_1 .. a_n}: phi = sum_p a_p r^(2p)  (phase/radial.py)
  * 1 / k0 per wavelength is derived at upload from the table's wavelength list.  A table with a phase surface
  * has bwd_supported = 0 and olb_table_upload_batch rejects it (OLB_ERR_UNSUPPORTED).
+ *
+ * GRATING is the ruled grating, DiffractiveInteractionModel (optiland/interactions/diffractive_model.py:28-61,
+ * RealRays.gratingdiffract), on OLB_GEOM_PLANE (PlaneGrating) or OLB_GEOM_STANDARD with a finite radius
+ * (StandardGratingGeometry); the geometry intersects and has its normal exactly as Plane / StandardGeometry.
+ * Block at pool[phase_off]: {1.0, 3, m, d, alpha} (the phase block's framing: "efficiency" exactly 1, three
+ * terms): order m, period d in micrometres (finite, non-zero, either sign), groove orientation alpha in radians.
+ * In the local frame, with the geometry's normal n and lambda in micrometres:
+ *     grating vector f = (-sin alpha, cos alpha, 0)                     on a plane
+ *                    f = -normalise(n x t), t = (1, tan alpha, dz/dx along the groove)   on a conic
+ *     n := sign(d0 . n) n   (aligned with the ray as refraction does; sign(0) = 0)
+ *     a = n1 d0 + g f,  g = m lambda sqrt(fx^2 + fy^2) / d
+ *     T = a |n|^2 - (a . n) n,   Q = n2^2 |n|^2 - |a x n|^2
+ *     d := normalise(+-T + sign(d) sqrt(Q) n)    (+ transmission, - reflection; n2 is material_post's index,
+ *                                                 for a mirror the medium before the surface)
+ * then the coating step with the unaligned normal, as for refraction.  Four behaviours of the reference are
+ * reproduced as they are:
+ *   1. a reflective grating returns the NEGATIVE of the physical reflected direction (the next surface is
+ *      reached with t < 0; the OPD stays positive through |t n|);
+ *   2. an evanescent order (Q < 0) gives NaN direction cosines and leaves the intensity unchanged (the NaN then
+ *      travels in band, as a missed surface does);
+ *   3. the grating adds no OPD term;
+ *   4. SimpleCoating scales i by R or T; FresnelCoating and polarized rays update P from d0 and the new d.
+ * A grating table also has bwd_supported = 0 and olb_table_upload_batch rejects it.
  */
 #define OLB_INTERACT_REFRACT        0
 #define OLB_INTERACT_PHASE_CONSTANT 1
 #define OLB_INTERACT_PHASE_LINEAR   2
 #define OLB_INTERACT_PHASE_RADIAL   3
+#define OLB_INTERACT_GRATING        4
 #define OLB_MAX_PHASE_TERMS        16
 
 /* ---- aperture programs --------------------------------------------------
@@ -176,7 +200,7 @@ typedef struct OlbSurface {
   int32_t media_off;   /* pool offset of the 5 x n_wl media block             */
   int32_t aux0;        /* polynomial: number of columns (y powers)            */
   int32_t interaction; /* OLB_INTERACT_* (0: refractive / reflective)          */
-  int32_t phase_off;   /* pool offset of the phase-profile block (see above)  */
+  int32_t phase_off;   /* pool offset of the phase / grating block (see above) */
   double t[3];         /* effective translation                               */
   double R[9];         /* effective rotation, row-major                       */
   double radius;       /* geometry.radius (inf => plane branch of Standard)   */

@@ -29,7 +29,7 @@ def template_params(table: T.SurfaceTable) -> np.ndarray:
     if table.n_wl != 1:
         raise ValueError("batched tables support one wavelength")
     if any(s.interaction != T.INTERACT_REFRACT for s in table.surfaces):
-        raise ValueError("batched tables with phase-profile surfaces are not built")
+        raise ValueError("batched tables with phase-profile or grating surfaces are not built")
     p = np.zeros((table.num_surfaces, _lib.BP_COUNT))
     for s, spec in enumerate(table.surfaces):
         p[s, _lib.BP_TX:_lib.BP_TX + 3] = spec.t

@@ -972,6 +972,53 @@ OLB_HD void phase_interact(Ray<T>& r, const PrepSurface<T>& S, const T* pool, T 
 // size); KIND (0 plane, 1 sphere/conic closed form, 2 Newton family) is resolved by the caller
 // ONCE per surface, outside the per-ray loop, so the hot loop carries no geometry branches.
 enum { KIND_PLANE = 0, KIND_CONIC = 1, KIND_NEWTON = 2, KIND_ASPHERE = 3 };   // NEWTON: any family (generic loop); ASPHERE: even / odd only (fused loop)
+
+// Ruled-grating interaction (DiffractiveInteractionModel.interact_real_rays, diffractive_model.py:28-61, with
+// RealRays.gratingdiffract): the vector form of include/olb.h (OLB_INTERACT_GRATING), which is algebraically the
+// reference's expanded expression divided through by the projected period, so every term is O(1) in fp32.  (nx, ny,
+// nz) is the geometry's unaligned normal; `n1` is material_pre's index (NaN for an unknown wavelength).  KIND is
+// KIND_PLANE (PlaneGrating) or KIND_CONIC (StandardGratingGeometry).  The reference's quirks stay: a reflective
+// grating returns the negative of the physical direction, an evanescent order (Q < 0) leaves NaN direction cosines
+// and the intensity unchanged, and no OPD term is added.
+template <typename T, int KIND>
+OLB_HD void grating_interact(Ray<T>& r, const PrepSurface<T>& S, const T* pool, T nx, T ny, T nz, T n1) {
+  const T* gb = pool + S.phase_off + PH_P;
+  const T* wl = gb + GR_WL + 2 * (r.widx < 0 ? 0 : r.widx);
+  const T mld = wl[0], n2 = wl[1] + (n1 - n1);   // (n1 - n1: NaN for an unknown wavelength, 0 otherwise)
+  // grating vector f, from the unaligned normal (plane_grating.py:113-132, standard_grating.py:102-256)
+  T fx, fy, fz;
+  if (KIND == KIND_PLANE) {
+    fx = -gb[GR_SIN]; fy = gb[GR_COS]; fz = 0;
+  } else {
+    // groove tangent t = (1, tan a, dz/dx along the groove) with dz/dx = -(nx + tan a ny) / nz on the conic; scaled
+    // by -nz > 0 (the conic normal points to -z), which f = -normalise(n x t) does not see
+    const T ta = gb[GR_TAN];
+    const T tx = -nz, ty = -nz * ta, tz = o_fma(ta, ny, nx);
+    const T cx = o_fma(ny, tz, -nz * ty), cy = o_fma(nz, tx, -nx * tz), cz = o_fma(nx, ty, -ny * tx);
+    const T inv = -o_rsqrt(o_fma(cx, cx, o_fma(cy, cy, cz * cz)));
+    fx = cx * inv; fy = cy * inv; fz = cz * inv;
+  }
+  const T g = mld * o_sqrt(o_fma(fx, fx, fy * fy));   // m lambda / (d / sqrt(fx^2 + fy^2))
+  // normal aligned with the incoming ray (real_rays.py:535-571; sign(0) = 0, sign(NaN) = NaN)
+  const T dot = o_fma(r.L, nx, o_fma(r.M, ny, r.N * nz));
+  const T sg = dot > 0 ? (T)1 : (dot < 0 ? (T)-1 : dot);
+  const T mx = nx * sg, my = ny * sg, mz = nz * sg;
+  const T ax = o_fma(g, fx, n1 * r.L), ay = o_fma(g, fy, n1 * r.M), az = o_fma(g, fz, n1 * r.N);
+  const T nn = o_fma(mx, mx, o_fma(my, my, mz * mz));
+  const T adn = o_fma(ax, mx, o_fma(ay, my, az * mz));
+  // T = a |n|^2 - (a . n) n ;  Q = n2^2 |n|^2 - |a x n|^2
+  const T tvx = o_fma(ax, nn, -adn * mx), tvy = o_fma(ay, nn, -adn * my), tvz = o_fma(az, nn, -adn * mz);
+  const T qx = o_fma(ay, mz, -az * my), qy = o_fma(az, mx, -ax * mz), qz = o_fma(ax, my, -ay * mx);
+  const T Q = o_fma(n2 * n2, nn, -o_fma(qx, qx, o_fma(qy, qy, qz * qz)));
+  const T sq = gb[GR_SGN] * o_sqrt(Q);                  // NaN when evanescent (the reference's behaviour)
+  const T sv = (S.flags & OLB_SF_REFLECT) ? (T)-1 : (T)1;
+  const T kx = o_fma(sq, mx, sv * tvx), ky = o_fma(sq, my, sv * tvy), kz = o_fma(sq, mz, sv * tvz);
+  const T inv = o_rsqrt(o_fma(kx, kx, o_fma(ky, ky, kz * kz)));
+  r.L = kx * inv;
+  r.M = ky * inv;
+  r.N = kz * inv;
+}
+
 template <typename T, uint32_t FEAT, int KIND>
 OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bool from_global, int& status,
                            T* Pm = nullptr, int Pstride = 1) {
@@ -1045,7 +1092,14 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
   if constexpr ((FEAT & FEAT_PHASE) != 0) {
     // phase-profile surface (phase_interaction_model.py:45-132): replaces refract / reflect
     if (S.phase != OLB_INTERACT_REFRACT) {
-      phase_interact(r, S, pool, nx, ny, nz, med[MED_N1] + bad);
+      if constexpr ((FEAT & FEAT_GRATING) != 0 && (KIND == KIND_PLANE || KIND == KIND_CONIC)) {
+        // ruled grating (diffractive_model.py:28-61): upload admits it on planes and conics only; its block has
+        // efficiency 1, so the efficiency step below leaves i as the reference does
+        if (S.phase == OLB_INTERACT_GRATING) grating_interact<T, KIND>(r, S, pool, nx, ny, nz, med[MED_N1] + bad);
+        else phase_interact(r, S, pool, nx, ny, nz, med[MED_N1] + bad);
+      } else {
+        phase_interact(r, S, pool, nx, ny, nz, med[MED_N1] + bad);
+      }
       phase = true;
     }
   }

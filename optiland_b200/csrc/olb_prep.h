@@ -33,6 +33,7 @@ enum : uint32_t {
   FEAT_POL = 1u << 3,      // polarized rays (P matrix) / Fresnel coatings
   FEAT_FREEFORM = 1u << 4, // polynomial / Zernike / Chebyshev / biconic / toroidal / Forbes surfaces (with NEWTON)
   FEAT_PHASE = 1u << 5,    // a phase-profile surface (PhaseInteractionModel): runs the general kernel + this
+  FEAT_GRATING = 1u << 6,  // a ruled grating (DiffractiveInteractionModel): runs the general kernel + PHASE + this
 };
 
 // Prepared phase block per surface (PrepSurface::phase_off), elements of T:
@@ -41,6 +42,9 @@ enum : uint32_t {
 //   coefficients in r^2); then, per wavelength j, {1 / k0 = lambda_j * 1e-3 / (2 pi) (mm / rad), n2 of the
 //   interaction (n1 when reflective, phase_interaction_model.py:53-56)}.
 enum { PH_EFF = 0, PH_NT = 1, PH_P = 2 };
+// Prepared grating block (OLB_INTERACT_GRATING), from PH_P: {sin alpha, cos alpha, tan alpha, sign(d)}, then per
+// wavelength j {m lambda_j / d, n2 = material_post's index} (GR_WL + 2 j).
+enum { GR_SIN = 0, GR_COS = 1, GR_TAN = 2, GR_SGN = 3, GR_WL = 4 };
 
 struct PrepHeader {
   int32_t n_surf;
@@ -480,8 +484,39 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     else if (in.coating == OLB_COAT_FRESNEL) features |= FEAT_POL;
     else if (in.coating != OLB_COAT_NONE) { res.error = "unknown coating"; return res; }
 
-    // ---- phase-profile interaction (PhaseInteractionModel) ---------------------------------------
-    if (in.interaction != OLB_INTERACT_REFRACT) {
+    // ---- ruled grating (DiffractiveInteractionModel) ---------------------------------------------
+    if (in.interaction == OLB_INTERACT_GRATING) {
+      if (in.kind == OLB_GEOM_NOOP) { res.error = "grating interaction on an object surface"; return res; }
+      if (in.kind != OLB_GEOM_PLANE && in.kind != OLB_GEOM_STANDARD) {
+        res.error = "grating interaction on a geometry other than a plane or a conic"; return res;
+      }
+      if (in.kind == OLB_GEOM_STANDARD && !std::isfinite(in.radius)) {
+        res.error = "grating interaction on a conic with an infinite radius"; return res;
+      }
+      if (!in_pool(in.phase_off, 5)) { res.error = "grating block outside pool"; return res; }
+      const double* gb = tab.pool + in.phase_off;
+      if (!(gb[1] == 3.0)) { res.error = "bad grating block: wrong number of terms"; return res; }
+      if (!(gb[0] == 1.0)) { res.error = "bad grating block: efficiency must be exactly 1"; return res; }
+      const double m = gb[2], d = gb[3], alpha = gb[4];
+      if (!std::isfinite(m) || !std::isfinite(alpha)) { res.error = "bad grating block: non-finite order or angle"; return res; }
+      if (!std::isfinite(d) || d == 0) { res.error = "bad grating block: non-finite or zero period"; return res; }
+      o.phase = in.interaction;
+      o.phase_off = (int)pool.size();
+      pool.push_back(1.0);
+      pool.push_back(3.0);
+      pool.push_back(std::sin(alpha));
+      pool.push_back(std::cos(alpha));
+      pool.push_back(std::tan(alpha));
+      pool.push_back(d > 0 ? 1.0 : -1.0);
+      for (int j = 0; j < n_wl; ++j) {
+        pool.push_back(m * tab.wavelengths[j] / d);
+        pool.push_back(tab.pool[in.media_off + n_wl + j]);
+      }
+      while (pool.size() % 4) pool.push_back(0);
+      features |= FEAT_GRATING;
+      res.bwd_supported = false;       // the adjoint has no grating interaction
+    } else if (in.interaction != OLB_INTERACT_REFRACT) {
+      // ---- phase-profile interaction (PhaseInteractionModel) -------------------------------------
       if (in.interaction < OLB_INTERACT_PHASE_CONSTANT || in.interaction > OLB_INTERACT_PHASE_RADIAL) {
         res.error = "unknown interaction model"; return res;
       }
@@ -560,7 +595,7 @@ static BatchPrep prepare_batch(const OlbTable& tmpl, const double* params, int n
   const int S = tmpl.n_surfaces;
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].interaction != OLB_INTERACT_REFRACT) {
-      out.error = "batched tables with phase-profile surfaces are not built"; out.unsupported = true; return out;
+      out.error = "batched tables with phase-profile or grating surfaces are not built"; out.unsupported = true; return out;
     }
   std::vector<OlbSurface> surf(tmpl.surfaces, tmpl.surfaces + S);
   std::vector<double> pool(tmpl.pool, tmpl.pool + tmpl.pool_len);

@@ -855,6 +855,8 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       // lean polarized variants for the common systems: the general kernel's code does not fit the instruction
       // cache (no_instruction was the second largest stall of the Zernike + Fresnel configuration)
       const uint32_t g = features & ~FEAT_POL;
+      if (g & FEAT_GRATING)                                                                             // gratings (+ phase)
+        return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL>(a, stream);
       if (g & FEAT_PHASE) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_POL>(a, stream);  // phase profiles
       if (g == 0) return launch_instance<T, 1, FEAT_POL>(a, stream);                                   // planes / conics
       if ((g & ~(FEAT_NEWTON | FEAT_FREEFORM)) == 0)
@@ -864,7 +866,9 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       return fail(OLB_ERR_UNSUPPORTED, "polarized trace uses one ray per thread");
     }
   }
-  // phase-profile tables: the general kernel plus the phase interaction, one ray per thread for either caller RPT
+  // phase-profile tables: the general kernel plus the phase interaction, one ray per thread for either caller RPT;
+  // tables with a ruled grating (phase surfaces allowed beside it) add the grating interaction to that
+  if (features & FEAT_GRATING) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING>(a, stream);
   if (features & FEAT_PHASE) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE>(a, stream);
   if (features == 0) return launch_instance<T, RPT, 0u>(a, stream);
   if (features == FEAT_ROT) return launch_instance<T, RPT, FEAT_ROT>(a, stream);

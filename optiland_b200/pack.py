@@ -93,7 +93,8 @@ class _Prefetch:
             if cs is not None:
                 for k in ("x", "y", "z", "rx", "ry", "rz"):
                     self._add(getattr(cs, k, None))
-            for k in ("radius", "k", "norm_x", "norm_y", "norm_radius", "Ry", "ky", "R_rot", "k_yz"):
+            for k in ("radius", "k", "norm_x", "norm_y", "norm_radius", "Ry", "ky", "R_rot", "k_yz",
+                      "grating_order", "grating_period", "groove_orientation_angle"):
                 self._add(getattr(g, k, None))
             for k in ("coefficients", "coeffs_poly_y"):
                 c = getattr(g, k, None)
@@ -276,6 +277,29 @@ def pack_phase_profile(profile) -> tuple[int, np.ndarray, float]:
     return kind, np.array(terms, dtype=np.float64), _f(profile.efficiency)
 
 
+_GRATING_KINDS = {"PlaneGrating": T.GEOM_PLANE, "StandardGratingGeometry": T.GEOM_STANDARD}
+
+
+def pack_grating(geometry, iname: str) -> tuple[int, tuple[float, float, float]]:
+    """(geometry kind, (order, period in um, groove angle in rad)) of a ruled grating: a ``PlaneGrating`` or a
+    ``StandardGratingGeometry`` under a ``DiffractiveInteractionModel`` (optiland/interactions/diffractive_model.py).
+    Only these exact classes are accepted, as a pair: a subclass may override the grating vector or the diffraction."""
+    gname = _cls(geometry)
+    if gname not in _GRATING_KINDS:
+        raise UnsupportedSurface(f"{iname} on geometry {gname}")
+    if iname != "DiffractiveInteractionModel":
+        raise UnsupportedSurface(f"interaction model {iname} on grating geometry {gname}")
+    kind = _GRATING_KINDS[gname]
+    if kind == T.GEOM_STANDARD and not np.isfinite(_f(geometry.radius)):
+        # StandardGratingGeometry has no plane branch (its normal and grating vector are NaN there)
+        raise UnsupportedSurface("StandardGratingGeometry with an infinite radius")
+    period = _f(geometry.grating_period)
+    if not np.isfinite(period) or period == 0:
+        # the reference yields NaN directions for these; its own loop reproduces that
+        raise UnsupportedSurface(f"grating period {period}")
+    return kind, (_f(geometry.grating_order), period, _f(geometry.groove_orientation_angle))
+
+
 def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     """One Optiland ``Surface`` / ``ObjectSurface`` / ``ImageSurface`` -> ``SurfaceSpec``."""
     sname = _cls(surface)
@@ -288,13 +312,17 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
 
     g = surface.geometry
     gname = _cls(g)
-    if gname not in _GEOM_KINDS:
-        raise UnsupportedSurface(f"geometry {gname}")
-    kind = _GEOM_KINDS[gname]
-
     im = surface.interaction_model
     iname = _cls(im)
-    if iname not in ("RefractiveReflectiveModel", "PhaseInteractionModel"):
+    grating = None
+    if gname in _GRATING_KINDS or iname == "DiffractiveInteractionModel":
+        kind, grating = pack_grating(g, iname)
+    elif gname not in _GEOM_KINDS:
+        raise UnsupportedSurface(f"geometry {gname}")
+    else:
+        kind = _GEOM_KINDS[gname]
+
+    if grating is None and iname not in ("RefractiveReflectiveModel", "PhaseInteractionModel"):
         raise UnsupportedSurface(f"interaction model {iname}")
     if getattr(im, "bsdf", None) is not None:
         raise UnsupportedSurface("bsdf scatter")
@@ -307,6 +335,9 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     spec = T.SurfaceSpec(kind=kind, t=t_eff, R=R_eff, reflective=bool(im.is_reflective))
     if phase is not None:
         spec.interaction, spec.phase_terms, spec.phase_efficiency = phase
+    if grating is not None:
+        spec.interaction = T.INTERACT_GRATING
+        spec.grating_order, spec.grating_period, spec.grating_angle = grating
     if kind != T.GEOM_PLANE:
         spec.radius = _f(g.radius)
         spec.conic = _f(g.k)

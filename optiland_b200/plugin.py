@@ -593,7 +593,7 @@ def _live_params(surfaces, table, wavelength):
     for surf, spec in zip(surfaces, table.surfaces):
         vals = [zero] * GP_COUNT
         if spec.interaction != T.INTERACT_REFRACT:
-            return None          # phase-profile surfaces: the adjoint has no phase interaction
+            return None          # phase-profile and grating surfaces: the adjoint has neither interaction
         if spec.kind != T.GEOM_NOOP:
             g = surf.geometry
             cs = g.cs
@@ -724,6 +724,8 @@ def _wants_grad(backend, surfaces, rays=None) -> bool:
             continue
         cs = g.cs
         vals = [getattr(g, "radius", None), getattr(g, "k", None), cs.x, cs.y, cs.z, cs.rx, cs.ry, cs.rz]
+        # ruled-grating scalars (pack.pack_grating)
+        vals += [getattr(g, k, None) for k in ("grating_order", "grating_period", "groove_orientation_angle")]
         parent = getattr(cs, "reference_cs", None)
         while parent is not None:                    # nested frames: the pose depends on every level
             vals += [parent.x, parent.y, parent.z, parent.rx, parent.ry, parent.rz]

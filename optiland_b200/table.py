@@ -45,6 +45,7 @@ INTERACT_REFRACT = 0
 INTERACT_PHASE_CONSTANT = 1
 INTERACT_PHASE_LINEAR = 2
 INTERACT_PHASE_RADIAL = 3
+INTERACT_GRATING = 4
 MAX_PHASE_TERMS = 16
 _PHASE_TERMS = {INTERACT_PHASE_CONSTANT: 1, INTERACT_PHASE_LINEAR: 2}
 
@@ -121,6 +122,11 @@ class SurfaceSpec:
     interaction: int = INTERACT_REFRACT
     phase_terms: np.ndarray = field(default_factory=lambda: np.zeros(0))
     phase_efficiency: float = 1.0
+    # ruled grating (DiffractiveInteractionModel, INTERACT_GRATING on a plane or a finite-radius conic): the
+    # diffraction order, the period in micrometres and the groove orientation angle in radians
+    grating_order: float = 0.0
+    grating_period: float = float("inf")
+    grating_angle: float = 0.0
 
     def __post_init__(self):
         self.t = np.asarray(self.t, dtype=np.float64).reshape(3)
@@ -205,7 +211,14 @@ class SurfaceTable:
                 validate_aperture_program(s.aperture)
             if s.coating == COAT_FRESNEL and (s.coat_n1 is None or s.coat_n2 is None):
                 raise ValueError("Fresnel coating needs coat_n1/coat_n2")
-            if s.interaction != INTERACT_REFRACT:
+            if s.interaction == INTERACT_GRATING:
+                if s.kind not in (GEOM_PLANE, GEOM_STANDARD) or (s.kind == GEOM_STANDARD and not np.isfinite(s.radius)):
+                    raise ValueError("grating: only on a plane or a conic with a finite radius")
+                if not (np.isfinite(s.grating_period) and s.grating_period != 0):
+                    raise ValueError(f"grating: period {s.grating_period} must be finite and non-zero")
+                if not (np.isfinite(s.grating_order) and np.isfinite(s.grating_angle)):
+                    raise ValueError("grating: non-finite order or angle")
+            elif s.interaction != INTERACT_REFRACT:
                 nt = len(s.phase_terms)
                 if s.interaction not in (INTERACT_PHASE_CONSTANT, INTERACT_PHASE_LINEAR, INTERACT_PHASE_RADIAL):
                     raise ValueError(f"unknown interaction {s.interaction}")
@@ -268,7 +281,11 @@ class SurfaceTable:
             cn2 = s.coat_n2 if s.coat_n2 is not None else s.n2
             ints["media_off"][j] = push(np.concatenate([s.n1, s.n2, s.k1, cn1, cn2]))
             assert len(s.n1) == n_wl
-            if s.interaction != INTERACT_REFRACT:
+            if s.interaction == INTERACT_GRATING:
+                # the phase block's framing: "efficiency" 1 (the diffractive model has none), 3 terms {m, d, alpha}
+                ints["interaction"][j] = s.interaction
+                ints["phase_off"][j] = push(np.array([1.0, 3.0, s.grating_order, s.grating_period, s.grating_angle]))
+            elif s.interaction != INTERACT_REFRACT:
                 ints["interaction"][j] = s.interaction
                 ints["phase_off"][j] = push(np.concatenate([[s.phase_efficiency, float(len(s.phase_terms))], s.phase_terms]))
         for k, v in ints.items():
@@ -356,7 +373,11 @@ class SurfaceTable:
             coating = int(r["coating"])
             inter = int(r["interaction"])
             phase = {}
-            if inter != INTERACT_REFRACT:
+            if inter == INTERACT_GRATING:
+                p0 = int(r["phase_off"])
+                phase = dict(interaction=inter, grating_order=float(pool[p0 + 2]), grating_period=float(pool[p0 + 3]),
+                             grating_angle=float(pool[p0 + 4]))
+            elif inter != INTERACT_REFRACT:
                 p0 = int(r["phase_off"])
                 phase = dict(interaction=inter, phase_efficiency=float(pool[p0]),
                              phase_terms=pool[p0 + 2: p0 + 2 + int(pool[p0 + 1])].copy())
