@@ -87,6 +87,43 @@ extern "C" {
 #define OLB_COAT_SIMPLE    1   /* SimpleCoating: i *= T or R (optiland/coatings.py:164-237) */
 #define OLB_COAT_FRESNEL   2   /* FresnelCoating (optiland/coatings.py:362-386,
                                   optiland/jones.py:71-117); needs polarized rays       */
+#define OLB_COAT_THIN_FILM 3   /* ThinFilmCoating (coatings.py:544, thin_film/core.py)   */
+#define OLB_COAT_POLARIZER 4   /* PolarizerCoating (coatings.py:418, JonesLinearPolarizer) */
+#define OLB_COAT_RETARDER  5   /* RetarderCoating (coatings.py:450, JonesLinearRetarder) */
+#define OLB_MAX_FILM_LAYERS 32
+/*
+ * THIN_FILM, POLARIZER and RETARDER are BaseCoatingPolarized coatings (coatings.py:285-331): a Jones matrix J
+ * per ray, then P := O_out J O_in P with the basis s, p0, p1 of PolarizedRays.get_local_basis, i.e.
+ *     M[a][b] = s_a (J00 s_b + J01 p0_b) + p1_a (J10 s_b + J11 p0_b) + J22 k1_a k0_b.
+ * Like FresnelCoating they need polarized rays; for RealRays the update is a no-op.  Their block sits right
+ * after the surface's media block, at pool[media_off + 5 * n_wl]:
+ *   THIN_FILM : {L, d_1 .. d_L, then per wavelength j: n0, k0, ns, ks, (n_l, k_l) x L}, 0 <= L <=
+ *               OLB_MAX_FILM_LAYERS, thicknesses d_l in micrometres (finite, >= 0); n0 + i k0 and ns + i ks are the
+ *               stack's incident and substrate materials (ThinFilmStack, which the surface keeps equal to its own
+ *               materials).  Per ray and polarization, the transfer-matrix method of thin_film/core.py:_tmm_coh
+ *               with theta0 = aoi = arccos(clip(|n . k0|)) (the geometry's unaligned normal, the direction before
+ *               the interaction) and Y = 0.002654418729832701:
+ *                   X = nr^2 - k^2 - (n0~ sin theta0)^2 - 2 i nr k   (principal sqrt; n~ cos = sqrt(X))
+ *                   eta_s = Y sqrt(X),  eta_p = Y^2 conj(n~)^2 / eta_s,  delta_l = 2 pi d_l / lambda sqrt(X_l)
+ *                   [A B; C D] = prod_l [[cos delta, i sin delta / eta], [i eta sin delta, cos delta]]  (incident first)
+ *                   denom = eta0 (A + etas B) + C + etas D  (1e-30 when |denom| == 0)
+ *                   r = (eta0 A + eta0 etas B - C - etas D) / denom,   t = conj(2 eta0 / denom)
+ *               (the conjugate on t is the reference's); J = diag(r_s, -r_p, -1) on reflection and
+ *               diag(t_s, t_p, 1) on transmission.  A stack of zero layers is the bare interface of these formulas.
+ *   POLARIZER : {ax, ay, az}, the normalised axis (JonesLinearPolarizer.axis).  u_in = (a.s, a.p0), u_out =
+ *               (a.s, a.p1), each normalised (norm 0 -> 1); J = u_out u_in^T, J22 = 1.
+ *   RETARDER  : {d, ax, ay, az}: retardance and normalised fast axis (JonesLinearRetarder.retardance / .axis).
+ *               (us, up) = u_in;  J00 = e^{-id/2} us^2 + e^{id/2} up^2,  J01 = J10 = -2i sin(d/2) us up,
+ *               J11 = e^{id/2} us^2 + e^{-id/2} up^2,  J22 = 1.
+ * One deliberate difference: each layer's characteristic matrix is carried scaled by e^{-|Im delta|} (r does not see
+ * the scale; t is multiplied back by e^{-sum |Im delta|}).  Where the reference's cosh / sinh overflow -- a thick,
+ * strongly absorbing layer, e.g. 20 um with n = 0.2, k = 5 -- it returns NaN for every ray; the kernel returns the finite
+ * limit (r of the opaque stack, t -> 0).  Below that range both agree to rounding.
+ * The axis is dotted with s, p0 and p1 in the SURFACE'S LOCAL frame, although the reference's docstrings say
+ * "global coordinates" -- the reference's behaviour, reproduced.  Polarizer and retarder act the same on
+ * reflection and transmission.  A table with one of these coatings has bwd_supported = 0 and
+ * olb_table_upload_batch rejects it (OLB_ERR_UNSUPPORTED).
+ */
 
 /* ---- interaction models (OlbSurface.interaction) ------------------------
  * 0 is the refractive / reflective model (optiland/interactions/refractive_reflective_model.py).  The
@@ -186,7 +223,8 @@ extern "C" {
  *     pool[media_off + 3*n_wl + j] = coating n1 (FresnelCoating.material_pre)
  *     pool[media_off + 4*n_wl + j] = coating n2 (FresnelCoating.material_post)
  * evaluated on the host by the reference's own material classes
- * (optiland/materials/base.py:98-149).
+ * (optiland/materials/base.py:98-149).  A thin-film, polarizer or retarder coating's block follows at
+ * pool[media_off + 5*n_wl] (see OLB_COAT_THIN_FILM).
  */
 typedef struct OlbSurface {
   int32_t kind;        /* OLB_GEOM_*                                          */

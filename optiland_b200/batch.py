@@ -30,6 +30,8 @@ def template_params(table: T.SurfaceTable) -> np.ndarray:
         raise ValueError("batched tables support one wavelength")
     if any(s.interaction != T.INTERACT_REFRACT for s in table.surfaces):
         raise ValueError("batched tables with phase-profile or grating surfaces are not built")
+    if any(s.coating in T.JONES_COATINGS for s in table.surfaces):
+        raise ValueError("batched tables with thin-film, polarizer or retarder coatings are not built")
     p = np.zeros((table.num_surfaces, _lib.BP_COUNT))
     for s, spec in enumerate(table.surfaces):
         p[s, _lib.BP_TX:_lib.BP_TX + 3] = spec.t

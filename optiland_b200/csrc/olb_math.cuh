@@ -804,13 +804,111 @@ template <typename T> OLB_HD Cx<T> c_div(Cx<T> a, Cx<T> b) {
   return {(a.re * b.re + a.im * b.im) * d, (a.im * b.re - a.re * b.im) * d};
 }
 
+template <typename T> OLB_HD Cx<T> c_add(Cx<T> a, Cx<T> b) { return {a.re + b.re, a.im + b.im}; }
+template <typename T> OLB_HD Cx<T> c_sub(Cx<T> a, Cx<T> b) { return {a.re - b.re, a.im - b.im}; }
+template <typename T> OLB_HD Cx<T> c_rcp(Cx<T> a) {
+  T d = o_rcp(o_fma(a.re, a.re, a.im * a.im));
+  return {a.re * d, -a.im * d};
+}
+// Principal square root, computed without cancellation.  A zero imaginary part takes the upper branch: the
+// reference's X = nr^2 - k^2 - (n0 sin)^2 - 2i nr k never carries -0 there (0 - (+0) = +0 in numpy).
+template <typename T> OLB_HD Cx<T> c_sqrt(Cx<T> z) {
+  const T m = o_sqrt(o_fma(z.re, z.re, z.im * z.im));
+  if (z.re >= 0) {
+    const T t = o_sqrt((m + z.re) * (T)0.5);
+    return {t, t == 0 ? (T)0 : o_div(z.im, 2 * t)};
+  }
+  const T t = o_sqrt((m - z.re) * (T)0.5);
+  return {o_div(o_abs(z.im), 2 * t), z.im < 0 ? -t : t};
+}
+// sin(pi a), cos(pi a): the argument reduction of sincospi is exact and needs no reduction table in device memory
+#if defined(__CUDA_ARCH__)
+OLB_HD void o_sincospi(double a, double* s, double* c) { sincospi(a, s, c); }
+OLB_HD void o_sincospi(float a, float* s, float* c) { sincospif(a, s, c); }
+#else
+template <typename T> inline void o_sincospi(T a, T* s, T* c) {
+  const T r = a - 2 * std::rint(a / 2);   // exact: a - 2k, |r| <= 1
+  *s = std::sin((T)M_PI * r);
+  *c = std::cos((T)M_PI * r);
+}
+#endif
+
+// Thin-film stack (OLB_COAT_THIN_FILM; thin_film/core.py:_tmm_coh): the Jones diagonal (js, jp) of one ray for both
+// polarizations at once.  `hdr` is the prepared header (olb_prep.h, CO_*), `c2` = cos^2(aoi) (NaN for an unknown
+// wavelength).  The incident medium's own X0 = n0~^2 cos^2 is formed from c2 directly: written as n0~^2 - n0~^2 sin^2
+// it cancels near grazing incidence (in fp32 t_s was off by 2 % at 89.95 degrees).  Each characteristic matrix is carried scaled by e^{-|Im delta|} -- r is a ratio of degree-1 forms in
+// (A, B, C, D) and does not see the scale, t is multiplied back by e^{-sum |Im delta|} -- so an absorbing layer with
+// a large Im delta neither overflows cosh / sinh nor turns the products into inf / inf.
+template <typename T>
+OLB_HD void thin_film_jones(const T* hdr, int widx, T c2, bool reflect, Cx<T>& js, Cx<T>& jp) {
+  const int L = (int)hdr[CO_L];
+  const T* rec = hdr - (int)hdr[CO_BACK] + (int)hdr[CO_STRIDE] * widx;
+  const T Y = (T)FILM_Y, iY = (T)(1.0 / FILM_Y);
+  const T s2 = 1 - c2;
+  const T n0r = rec[0] * s2, n0i = rec[1] * s2;   // (n0~ sin theta0)^2
+  // X = A - (n0~ sin)^2 - iB, sqrt(X) = n~ cos theta;  eta_s = Y sqrt(X), eta_p = Y conj(n~)^2 / sqrt(X)
+  // incident medium: X0 = A0 - iB0 - (A0 + iB0) sin^2 = A0 cos^2 - i B0 (1 + sin^2)
+  const Cx<T> q0 = c_sqrt(Cx<T>{rec[0] * c2, (T)0 - rec[1] * (2 - c2)});
+  const Cx<T> qs = c_sqrt(Cx<T>{rec[2] - n0r, (T)0 - n0i - rec[3]});
+  const Cx<T> e0s = {Y * q0.re, Y * q0.im}, ess = {Y * qs.re, Y * qs.im};
+  const Cx<T> e0p = c_mul(Cx<T>{Y * rec[0], -Y * rec[1]}, c_rcp(q0));
+  const Cx<T> esp = c_mul(Cx<T>{Y * rec[2], -Y * rec[3]}, c_rcp(qs));
+  Cx<T> As = {1, 0}, Bs = {0, 0}, Cs = {0, 0}, Ds = {1, 0};
+  Cx<T> Ap = {1, 0}, Bp = {0, 0}, Cp = {0, 0}, Dp = {1, 0};
+  T E = 0;
+  for (int l = 0; l < L; ++l) {
+    const T* ly = rec + CO_REC + CO_LAYER * l;
+    const Cx<T> q = c_sqrt(Cx<T>{ly[1] - n0r, (T)0 - n0i - ly[2]});
+    // delta = 2 pi d / lambda * sqrt(X) = pi (dr + i di)
+    const T dr = ly[0] * q.re, di = (T)M_PI * (ly[0] * q.im);
+    T sr, cr;
+    o_sincospi(dr, &sr, &cr);
+    const T adi = o_abs(di), e = o_exp(-2 * adi);
+    const T ch = (1 + e) * (T)0.5, sh = (di < 0 ? (T)-0.5 : (T)0.5) * (1 - e);   // cosh, sinh times e^{-|di|}
+    E += adi;
+    const Cx<T> c = {cr * ch, -sr * sh};                // cos delta
+    const Cx<T> is = {-cr * sh, sr * ch};               // i sin delta
+    const Cx<T> iq = c_rcp(q);
+    // s: i sin / eta = i sin / (Y q),  i eta sin = i sin Y q
+    const Cx<T> mBs = c_mul(is, Cx<T>{iq.re * iY, iq.im * iY}), mCs = c_mul(is, Cx<T>{Y * q.re, Y * q.im});
+    // p: i sin / eta_p = i sin q / (Y conj(n~)^2),  i eta_p sin = i sin Y conj(n~)^2 / q
+    const Cx<T> mBp = c_mul(is, c_mul(q, Cx<T>{ly[3], ly[4]}));
+    const Cx<T> mCp = c_mul(is, c_mul(Cx<T>{Y * ly[1], -Y * ly[2]}, iq));
+    Cx<T> a = c_add(c_mul(As, c), c_mul(Bs, mCs)), b = c_add(c_mul(As, mBs), c_mul(Bs, c));
+    Cx<T> cc = c_add(c_mul(Cs, c), c_mul(Ds, mCs)), d = c_add(c_mul(Cs, mBs), c_mul(Ds, c));
+    As = a; Bs = b; Cs = cc; Ds = d;
+    a = c_add(c_mul(Ap, c), c_mul(Bp, mCp)); b = c_add(c_mul(Ap, mBp), c_mul(Bp, c));
+    cc = c_add(c_mul(Cp, c), c_mul(Dp, mCp)); d = c_add(c_mul(Cp, mBp), c_mul(Dp, c));
+    Ap = a; Bp = b; Cp = cc; Dp = d;
+  }
+  const T sc = o_exp(-E);
+  // denom = eta0 (A + etas B) + C + etas D ;  r = (eta0 (A + etas B) - C - etas D) / denom ;  t = conj(2 eta0 / denom)
+  auto rt = [&](Cx<T> e0, Cx<T> es, Cx<T> A, Cx<T> B, Cx<T> C, Cx<T> D, Cx<T>& rr, Cx<T>& tt) {
+    const Cx<T> u = c_mul(e0, c_add(A, c_mul(es, B))), v = c_add(C, c_mul(es, D));
+    Cx<T> den = c_add(u, v);
+    if (den.re == 0 && den.im == 0) den = {(T)1e-30, (T)0};
+    const Cx<T> id = c_rcp(den);
+    rr = c_mul(c_sub(u, v), id);
+    const Cx<T> t2 = c_mul(Cx<T>{2 * e0.re, 2 * e0.im}, id);
+    tt = {t2.re * sc, -t2.im * sc};
+  };
+  Cx<T> rs, ts, rp, tp;
+  rt(e0s, ess, As, Bs, Cs, Ds, rs, ts);
+  rt(e0p, esp, Ap, Bp, Cp, Dp, rp, tp);
+  if (reflect) { js = rs; jp = {-rp.re, -rp.im}; }
+  else { js = ts; jp = tp; }
+}
+
 // P := O_out * J * O_in * P for one ray.  k0 = (L0,M0,N0), k1 = (L,M,N) in the surface's local
 // frame (the reference mixes local frames across tilted surfaces; reproduced).  `cosi` = |n.k0|.
 // The matrix lives wherever the caller keeps it: element q (q = 2 (3 row + col) + {0: Re, 1: Im}) at P[q * ps] --
 // the kernel holds it in shared memory ([q][thread], conflict-free, ps = block size) so that the 18 values are
 // not carried in registers across the geometry step; the host check passes Ray::P with ps = 1.
-template <typename T>
-OLB_HD void polar_update(Ray<T>& r, T* P, int ps, const PrepSurface<T>& S, T ncoat, T cosi) {
+// JONES (kernels of tables with a thin-film / polarizer / retarder coating) adds those coatings and the general 2x2
+// Jones block; `pool` and `bad` (NaN for an unknown wavelength) are read by it only.
+template <typename T, bool JONES = false>
+OLB_HD void polar_update(Ray<T>& r, T* P, int ps, const PrepSurface<T>& S, T ncoat, T cosi, const T* pool = nullptr,
+                         T bad = 0) {
   const T k0[3] = {r.L0, r.M0, r.N0}, k1[3] = {r.L, r.M, r.N};
   // s = k0 x k1, with the reference's fallback when k0 || k1 (polarized_rays.py:151-163).  At an
   // index-matched surface (the image surface: n1 == n2) k1 == k0 and s must come out exactly 0.
@@ -849,8 +947,54 @@ OLB_HD void polar_update(Ray<T>& r, T* P, int ps, const PrepSurface<T>& S, T nco
       jp = c_div(Cx<T>{2 * n * c, (T)0}, Cx<T>{n2c.re + root.re, root.im});
     }
   }
-  // M[r][c] = s_r js s_c + p1_r jp p0_c + k1_r jk k0_c      (o_out @ J @ o_in)
   Cx<T> Mx[9];
+  if constexpr (JONES) {
+    // general Jones block (J00 J01; J10 J11), J22 = jk
+    Cx<T> j01 = {(T)0, (T)0}, j10 = {(T)0, (T)0};
+    const T* hdr = pool + S.media_off - CO_HDR;
+    if (S.coating == OLB_COAT_THIN_FILM) {
+      // aoi = arccos(clip(|n.k0|)): cos^2(aoi) = c^2
+      const T c = cosi > (T)1 ? (T)1 : cosi;
+      const bool refl = (S.flags & OLB_SF_REFLECT) != 0;
+      thin_film_jones(hdr, r.widx < 0 ? 0 : r.widx, c * c + bad, refl, js, jp);
+      jk = refl ? (T)-1 : (T)1;
+    } else if (S.coating == OLB_COAT_POLARIZER || S.coating == OLB_COAT_RETARDER) {
+      // (a.s, a.p0) and (a.s, a.p1), each normalised, a zero norm taken as 1 (jones.py: JonesLinearPolarizer /
+      // JonesLinearRetarder); both act the same on reflection and transmission
+      const T ax = hdr[CO_AX], ay = hdr[CO_AX + 1], az = hdr[CO_AX + 2];
+      const T ts = o_fma(ax, s[0], o_fma(ay, s[1], az * s[2]));
+      const T tpi = o_fma(ax, p0[0], o_fma(ay, p0[1], az * p0[2]));
+      T ni = o_sqrt(o_fma(ts, ts, tpi * tpi));
+      if (ni == 0) ni = 1;
+      const T usi = o_div(ts, ni), upi = o_div(tpi, ni);
+      if (S.coating == OLB_COAT_POLARIZER) {
+        const T tpo = o_fma(ax, p1[0], o_fma(ay, p1[1], az * p1[2]));
+        T no = o_sqrt(o_fma(ts, ts, tpo * tpo));
+        if (no == 0) no = 1;
+        const T uso = o_div(ts, no), upo = o_div(tpo, no);
+        js = {uso * usi, (T)0}; j01 = {uso * upi, (T)0}; j10 = {upo * usi, (T)0}; jp = {upo * upi, (T)0};
+      } else {
+        // e^{-+id/2} us^2 + e^{+-id/2} up^2 = cos(d/2) (us^2 + up^2) -+ i sin(d/2) (us^2 - up^2)
+        const T ch = hdr[CO_COS], sh = hdr[CO_SIN];
+        const T u2 = usi * usi, v2 = upi * upi;
+        js = {ch * (u2 + v2), -sh * (u2 - v2)};
+        jp = {ch * (u2 + v2), sh * (u2 - v2)};
+        j01 = {(T)0, -2 * sh * usi * upi};
+        j10 = j01;
+      }
+      jk = 1;
+    }
+    // M[a][b] = s_a (J00 s_b + J01 p0_b) + p1_a (J10 s_b + J11 p0_b) + J22 k1_a k0_b
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      const Cx<T> u = {o_fma(js.re, s[b], j01.re * p0[b]), o_fma(js.im, s[b], j01.im * p0[b])};
+      const Cx<T> v = {o_fma(j10.re, s[b], jp.re * p0[b]), o_fma(j10.im, s[b], jp.im * p0[b])};
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+        Mx[3 * a + b] = {o_fma(s[a], u.re, o_fma(p1[a], v.re, k1[a] * k0[b] * jk)), o_fma(s[a], u.im, p1[a] * v.im)};
+    }
+  } else {
+  // M[r][c] = s_r js s_c + p1_r jp p0_c + k1_r jk k0_c      (o_out @ J @ o_in)
 #pragma unroll
   for (int a = 0; a < 3; ++a)
 #pragma unroll
@@ -858,6 +1002,7 @@ OLB_HD void polar_update(Ray<T>& r, T* P, int ps, const PrepSurface<T>& S, T nco
       T ss = s[a] * s[b], pp = p1[a] * p0[b], kk = k1[a] * k0[b] * jk;
       Mx[3 * a + b] = {o_fma(ss, js.re, o_fma(pp, jp.re, kk)), o_fma(ss, js.im, pp * jp.im)};
     }
+  }
   // P := M P, column by column
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -1136,7 +1281,8 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
     if (S.coating != OLB_COAT_SIMPLE)
       // (Pm is the caller's matrix storage -- never a pointer into `r`: taking r.P's address here would force the
       // whole ray state into local memory in the kernel)
-      polar_update(r, Pm, Pstride, S, med[MED_CN] + bad, o_abs(o_fma(r.L0, nx, o_fma(r.M0, ny, r.N0 * nz))));
+      polar_update<T, (FEAT & FEAT_JONES) != 0>(r, Pm, Pstride, S, med[MED_CN] + bad,
+                                                o_abs(o_fma(r.L0, nx, o_fma(r.M0, ny, r.N0 * nz))), pool, bad);
   }
   // -- phase profile efficiency (phase_interaction_model.py:129-130)
   if constexpr ((FEAT & FEAT_PHASE) != 0) {

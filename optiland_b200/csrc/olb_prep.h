@@ -34,7 +34,21 @@ enum : uint32_t {
   FEAT_FREEFORM = 1u << 4, // polynomial / Zernike / Chebyshev / biconic / toroidal / Forbes surfaces (with NEWTON)
   FEAT_PHASE = 1u << 5,    // a phase-profile surface (PhaseInteractionModel): runs the general kernel + this
   FEAT_GRATING = 1u << 6,  // a ruled grating (DiffractiveInteractionModel): runs the general kernel + PHASE + this
+  FEAT_JONES = 1u << 7,    // a thin-film / polarizer / retarder coating (with POL): the general polarized kernel +
+                           // PHASE + GRATING + this
 };
+
+// Prepared block of a thin-film / polarizer / retarder coating: it sits right BEFORE the surface's prepared media
+// block, so the kernel finds it from PrepSurface::media_off alone.  Its CO_HDR-element header ends at media_off:
+//   thin film : {L, record stride, n_wl * stride, ...}; the records of wavelengths 0 .. n_wl-1 precede the header
+//               (record j at header - n_wl * stride + j * stride): {A0, B0, As, Bs} of the incident medium and the
+//               substrate, then per layer {2 d / lambda, A, B, Re, Im of 1 / (Y conj(n~)^2)}, where for n~ = n + ik
+//               A = n^2 - k^2 and B = 2 n k (so n~^2 = A + iB and conj(n~)^2 = A - iB)
+//   polarizer : {ax, ay, az}
+//   retarder  : {ax, ay, az, cos(d/2), sin(d/2)}
+enum { CO_HDR = 8, CO_L = 0, CO_STRIDE = 1, CO_BACK = 2, CO_AX = 0, CO_COS = 3, CO_SIN = 4, CO_REC = 4, CO_LAYER = 5 };
+// thin-film admittance of free space, sqrt(eps0 / mu0) in siemens (thin_film/core.py:_admittance)
+constexpr double FILM_Y = 0.002654418729832701370374020517935;
 
 // Prepared phase block per surface (PrepSurface::phase_off), elements of T:
 //   [PH_EFF] efficiency, [PH_NT] number of profile terms n, then from PH_P the profile terms:
@@ -464,6 +478,66 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
 
     // ---- media -----------------------------------------------------------------
     if (!in_pool(in.media_off, 5 * n_wl)) { res.error = "media block outside pool"; return res; }
+
+    // ---- thin-film / polarizer / retarder coating: its prepared block goes right before the media block ------
+    if (in.coating >= OLB_COAT_THIN_FILM && in.coating <= OLB_COAT_RETARDER) {
+      if (in.kind == OLB_GEOM_NOOP) { res.error = "polarizing coating on an object surface"; return res; }
+      const int cb = in.media_off + 5 * n_wl;
+      std::vector<double> hdr(CO_HDR, 0.0);
+      if (in.coating == OLB_COAT_THIN_FILM) {
+        if (!in_pool(cb, 1)) { res.error = "thin-film block outside pool"; return res; }
+        const double Ld = tab.pool[cb];
+        const int L = (int)Ld;
+        if (!(Ld == (double)L) || L < 0 || L > OLB_MAX_FILM_LAYERS) {
+          res.error = "bad thin-film block: number of layers out of range"; return res;
+        }
+        if (!in_pool(cb, 1 + L + n_wl * (4 + 2 * L))) { res.error = "thin-film block outside pool"; return res; }
+        const double* d = tab.pool + cb + 1;
+        for (int l = 0; l < L; ++l)
+          if (!std::isfinite(d[l]) || d[l] < 0) { res.error = "bad thin-film block: thickness not finite and >= 0"; return res; }
+        int stride = CO_REC + CO_LAYER * L;
+        while (stride % 4) ++stride;
+        for (int j = 0; j < n_wl; ++j) {
+          const double* w = tab.pool + cb + 1 + L + j * (4 + 2 * L);
+          const size_t r0 = pool.size();
+          pool.push_back(w[0] * w[0] - w[1] * w[1]);   // incident n0~^2 = A0 + i B0
+          pool.push_back(2.0 * w[0] * w[1]);
+          pool.push_back(w[2] * w[2] - w[3] * w[3]);   // substrate
+          pool.push_back(2.0 * w[2] * w[3]);
+          const double k0 = 2.0 / tab.wavelengths[j];     // phase thickness / pi per unit sqrt(X) and thickness
+          for (int l = 0; l < L; ++l) {
+            const double n = w[4 + 2 * l], k = w[5 + 2 * l];
+            const double A = n * n - k * k, B = 2.0 * n * k;
+            const double m2 = FILM_Y * (A * A + B * B);   // 1 / (Y (A - iB)) = (A + iB) / (Y (A^2 + B^2))
+            pool.push_back(k0 * d[l]);
+            pool.push_back(A);
+            pool.push_back(B);
+            pool.push_back(A / m2);
+            pool.push_back(B / m2);
+          }
+          while (pool.size() - r0 < (size_t)stride) pool.push_back(0);
+        }
+        hdr[CO_L] = L;
+        hdr[CO_STRIDE] = stride;
+        hdr[CO_BACK] = (double)stride * n_wl;
+      } else {
+        const int na = in.coating == OLB_COAT_POLARIZER ? 3 : 4;
+        if (!in_pool(cb, na)) { res.error = "polarizer / retarder block outside pool"; return res; }
+        const double* a = tab.pool + cb + (na - 3);
+        const double norm = std::sqrt(a[0] * a[0] + a[1] * a[1] + a[2] * a[2]);
+        if (!std::isfinite(norm) || norm == 0) { res.error = "bad polarizer / retarder block: axis not finite and non-zero"; return res; }
+        for (int q = 0; q < 3; ++q) hdr[CO_AX + q] = a[q];
+        if (in.coating == OLB_COAT_RETARDER) {
+          const double dr = tab.pool[cb];
+          if (!std::isfinite(dr)) { res.error = "bad retarder block: non-finite retardance"; return res; }
+          hdr[CO_COS] = std::cos(dr / 2);
+          hdr[CO_SIN] = std::sin(dr / 2);
+        }
+      }
+      pool.insert(pool.end(), hdr.begin(), hdr.end());
+      features |= FEAT_POL | FEAT_JONES;
+      res.bwd_supported = false;       // the adjoint has no polarization
+    }
     o.media_off = (int)pool.size();
     bool absorbing = false;
     for (int j = 0; j < n_wl; ++j) {
@@ -482,7 +556,9 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     else o.flags &= ~uint32_t(OLB_SF_ABSORBING);
     if (in.coating == OLB_COAT_SIMPLE) features |= FEAT_EXTRA;
     else if (in.coating == OLB_COAT_FRESNEL) features |= FEAT_POL;
-    else if (in.coating != OLB_COAT_NONE) { res.error = "unknown coating"; return res; }
+    else if (in.coating != OLB_COAT_NONE && !(in.coating >= OLB_COAT_THIN_FILM && in.coating <= OLB_COAT_RETARDER)) {
+      res.error = "unknown coating"; return res;
+    }
 
     // ---- ruled grating (DiffractiveInteractionModel) ---------------------------------------------
     if (in.interaction == OLB_INTERACT_GRATING) {
@@ -596,6 +672,10 @@ static BatchPrep prepare_batch(const OlbTable& tmpl, const double* params, int n
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].interaction != OLB_INTERACT_REFRACT) {
       out.error = "batched tables with phase-profile or grating surfaces are not built"; out.unsupported = true; return out;
+    }
+  for (int s = 0; s < S && tmpl.surfaces; ++s)
+    if (tmpl.surfaces[s].coating >= OLB_COAT_THIN_FILM && tmpl.surfaces[s].coating <= OLB_COAT_RETARDER) {
+      out.error = "batched tables with thin-film, polarizer or retarder coatings are not built"; out.unsupported = true; return out;
     }
   std::vector<OlbSurface> surf(tmpl.surfaces, tmpl.surfaces + S);
   std::vector<double> pool(tmpl.pool, tmpl.pool + tmpl.pool_len);

@@ -855,7 +855,9 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       // lean polarized variants for the common systems: the general kernel's code does not fit the instruction
       // cache (no_instruction was the second largest stall of the Zernike + Fresnel configuration)
       const uint32_t g = features & ~FEAT_POL;
-      if (g & FEAT_GRATING)                                                                             // gratings (+ phase)
+      if (g & FEAT_JONES)        // thin-film / polarizer / retarder coatings, on any surface (DOEs and gratings too)
+        return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES>(a, stream);
+      if (g & FEAT_GRATING)                                                                            // gratings (+ phase)
         return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL>(a, stream);
       if (g & FEAT_PHASE) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_POL>(a, stream);  // phase profiles
       if (g == 0) return launch_instance<T, 1, FEAT_POL>(a, stream);                                   // planes / conics

@@ -122,7 +122,17 @@ class _Prefetch:
                         stack.append(u)
                     else:
                         self._add(u)
-            for mat in (getattr(surf, "material_pre", None), getattr(surf, "material_post", None)):
+            mats = [getattr(surf, "material_pre", None), getattr(surf, "material_post", None)]
+            coating = getattr(getattr(surf, "interaction_model", None), "coating", None)
+            if _cls(coating) == "ThinFilmCoating":
+                try:
+                    mats += _film_materials(coating)
+                    self._add([layer.thickness_um for layer in coating.jones.stack.layers])
+                except Exception:
+                    pass
+            elif _cls(coating) == "RetarderCoating":
+                self._add(getattr(getattr(coating, "jones", None), "retardance", None))
+            for mat in mats:
                 if mat is None:
                     continue
                 for wl in self.wavelengths:
@@ -300,6 +310,67 @@ def pack_grating(geometry, iname: str) -> tuple[int, tuple[float, float, float]]
     return kind, (_f(geometry.grating_order), period, _f(geometry.groove_orientation_angle))
 
 
+# BaseCoatingPolarized coatings with their own Jones model (optiland/coatings.py:418-580): coating class -> the exact
+# Jones class its ``jones`` property must return
+_JONES_COATINGS = {"ThinFilmCoating": "JonesThinFilm", "PolarizerCoating": "JonesLinearPolarizer",
+                   "RetarderCoating": "JonesLinearRetarder"}
+
+
+def _jones_axis(jones) -> np.ndarray:
+    axis = _arr(jones.axis).astype(np.float64).reshape(-1)
+    if axis.size != 3 or not np.all(np.isfinite(axis)) or not np.any(axis != 0):
+        raise UnsupportedSurface(f"{_cls(jones)} axis {axis.tolist()}")
+    return axis
+
+
+def _film_materials(coating):
+    """The materials a ``ThinFilmCoating`` reads per wavelength: the stack's incident and substrate materials and
+    every layer's (thin_film/core.py:_tmm_coh)."""
+    stack = coating.jones.stack
+    return [stack.incident_material, stack.substrate_material] + [layer.material for layer in stack.layers]
+
+
+def pack_jones_coating(spec: T.SurfaceSpec, coating, wavelengths) -> None:
+    """Thin-film, polarizer or retarder coating -> ``spec`` (include/olb.h OLB_COAT_THIN_FILM ...).  Only the exact
+    coating classes with their own Jones classes are accepted: a subclass may override the Jones matrix.  What is read
+    is what ``coating.jones.calculate_matrix`` reads: the Jones model's stack, axis and retardance."""
+    cname = _cls(coating)
+    jones = coating.jones
+    if _cls(jones) != _JONES_COATINGS[cname]:
+        raise UnsupportedSurface(f"{cname} with Jones model {_cls(jones)}")
+    if cname == "ThinFilmCoating":
+        stack = jones.stack
+        if _cls(stack) != "ThinFilmStack":
+            raise UnsupportedSurface(f"thin-film stack class {_cls(stack)}")
+        layers = list(stack.layers)
+        if len(layers) > T.MAX_FILM_LAYERS:
+            raise UnsupportedSurface(f"thin-film stack with more than {T.MAX_FILM_LAYERS} layers")
+        if any(_cls(layer) != "Layer" for layer in layers):
+            raise UnsupportedSurface("thin-film layer class other than Layer")
+        d = np.array([_f(layer.thickness_um) for layer in layers], dtype=np.float64)
+        if not np.all(np.isfinite(d)) or np.any(d < 0):
+            raise UnsupportedSurface(f"thin-film thicknesses {d.tolist()}")
+        spec.coating = T.COAT_THIN_FILM
+        spec.film_thickness = d
+        n_wl = len(wavelengths)
+        spec.film_n = np.array([_index_table(layer.material, wavelengths, "n") for layer in layers]).reshape(-1, n_wl)
+        spec.film_k = np.array([_index_table(layer.material, wavelengths, "k") for layer in layers]).reshape(-1, n_wl)
+        spec.film_n0 = _index_table(stack.incident_material, wavelengths, "n")
+        spec.film_k0 = _index_table(stack.incident_material, wavelengths, "k")
+        spec.film_ns = _index_table(stack.substrate_material, wavelengths, "n")
+        spec.film_ks = _index_table(stack.substrate_material, wavelengths, "k")
+    elif cname == "PolarizerCoating":
+        spec.coating = T.COAT_POLARIZER
+        spec.jones_axis = _jones_axis(jones)      # normalised once at construction (jones.py:128-130)
+    else:
+        retardance = _f(jones.retardance)
+        if not np.isfinite(retardance):
+            raise UnsupportedSurface(f"retardance {retardance}")
+        spec.coating = T.COAT_RETARDER
+        spec.retardance = retardance
+        spec.jones_axis = _jones_axis(jones)
+
+
 def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     """One Optiland ``Surface`` / ``ObjectSurface`` / ``ImageSurface`` -> ``SurfaceSpec``."""
     sname = _cls(surface)
@@ -406,6 +477,8 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
             spec.coating = T.COAT_FRESNEL
             spec.coat_n1 = _index_table(coating.material_pre, wavelengths, "n")
             spec.coat_n2 = _index_table(coating.material_post, wavelengths, "n")
+        elif cname in _JONES_COATINGS:
+            pack_jones_coating(spec, coating, wavelengths)
         else:
             raise UnsupportedSurface(f"coating {cname}")
     spec.__post_init__()

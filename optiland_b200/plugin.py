@@ -742,6 +742,10 @@ def _wants_grad(backend, surfaces, rays=None) -> bool:
             pc = getattr(pp, "coefficients", None)
             if pc is not None:
                 vals += [pc] if hasattr(pc, "requires_grad") else list(np.ravel(np.asarray(pc, dtype=object)))
+        jones = getattr(getattr(getattr(surf, "interaction_model", None), "coating", None), "jones", None)
+        if jones is not None:                        # thin-film thicknesses, retardance (pack.pack_jones_coating)
+            vals += [getattr(layer, "thickness_um", None) for layer in getattr(getattr(jones, "stack", None), "layers", [])]
+            vals += [getattr(jones, "retardance", None), getattr(jones, "axis", None)]
         if any(rg(v) for v in vals):
             return True
     return False
@@ -815,6 +819,9 @@ def _try_trace(backend, surfaces, rays, table_builder) -> bool:
     if not polarized and any(s.coating == T.COAT_FRESNEL for s in table.surfaces):
         # the reference raises for this combination (ray_generator.py:90-94)
         return _decline("Fresnel coating with unpolarized rays")
+    if not polarized and any(s.coating in T.JONES_COATINGS for s in table.surfaces):
+        # the reference's ray generator raises for these too (ray_generator.py:90-94); RealRays pass them unchanged
+        return _decline("thin-film, polarizer or retarder coating with unpolarized rays")
     launch_dir = (rays.L, rays.M, rays.N)
     if _wants_grad(backend, surfaces, rays):
         # gradients wanted: the records must be autograd outputs of the live parameter tensors
@@ -920,7 +927,7 @@ def install(engine=None, alias: str | None = None) -> None:
                 _prepare(engine, table, Px.device)
             except _PACK_ERRORS as e:
                 return _fused_decline(f"unsupported: {e}")
-            if not polarized and any(s.coating == T.COAT_FRESNEL for s in table.surfaces):
+            if not polarized and any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces):
                 return None          # the reference raises for this combination (ray_generator.py:90-94)
             if table.surfaces[0].kind != T.GEOM_NOOP:
                 return _fused_decline("first surface is not an object surface")
@@ -1041,7 +1048,7 @@ def install(engine=None, alias: str | None = None) -> None:
                     aff["vig"] = vig
             except _PACK_ERRORS as e:
                 return _fused_decline(f"unsupported: {e}")
-            if not polarized and any(s.coating == T.COAT_FRESNEL for s in table.surfaces):
+            if not polarized and any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces):
                 return None          # the reference raises (ray_generator.py:90-94)
             if table.surfaces[0].kind != T.GEOM_NOOP:
                 return _fused_decline("first surface is not an object surface")
@@ -1110,7 +1117,7 @@ def install(engine=None, alias: str | None = None) -> None:
                 _prepare(engine, table, Px.device)
             except _PACK_ERRORS as e:
                 return _fused_decline(f"wavefront unsupported: {e}")
-            if not polarized and any(s.coating == T.COAT_FRESNEL for s in table.surfaces):
+            if not polarized and any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces):
                 return None
             # steps 1-2, the reference's own code on ONE ray (strategy.py:160-170)
             chief = optic.trace_generic(*field, Px=0.0, Py=0.0, wavelength=wavelength)

@@ -144,7 +144,7 @@ def _fused_inputs(P, backend, be, optic, Hx, Hy, wavelength, num_rays, distribut
         P._prepare(engine, table, Px.device)
     except P._PACK_ERRORS as e:
         return P._fused_decline(f"spot moments unsupported: {e}")
-    if any(s.coating == T.COAT_FRESNEL for s in table.surfaces) or table.surfaces[0].kind != T.GEOM_NOOP:
+    if any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces) or table.surfaces[0].kind != T.GEOM_NOOP:
         return None
     return (table, Px, Py, pupil_affine(sc)), apod
 

@@ -40,6 +40,20 @@ SF_NORECORD = 1 << 4
 COAT_NONE = 0
 COAT_SIMPLE = 1
 COAT_FRESNEL = 2
+COAT_THIN_FILM = 3
+COAT_POLARIZER = 4
+COAT_RETARDER = 5
+MAX_FILM_LAYERS = 32
+# prepared thin-film records of one table, in elements (olb_prep.h: per surface n_wl records of 4 + 5 L, rounded up to 4,
+# plus an 8-element header).  They are staged in shared memory with the rest of the table; 8192 elements (64 KiB in fp64)
+# keeps the polarized kernel well inside the per-block limit with room for the surfaces and the P-matrix slots.
+MAX_FILM_ELEMENTS = 8192
+
+
+def film_elements(L: int, n_wl: int) -> int:
+    return n_wl * (-(-(4 + 5 * L) // 4) * 4) + 8
+JONES_COATINGS = (COAT_THIN_FILM, COAT_POLARIZER, COAT_RETARDER)   # their own Jones model (include/olb.h)
+POLARIZING_COATINGS = (COAT_FRESNEL,) + JONES_COATINGS               # need polarized rays
 
 INTERACT_REFRACT = 0
 INTERACT_PHASE_CONSTANT = 1
@@ -127,6 +141,18 @@ class SurfaceSpec:
     grating_order: float = 0.0
     grating_period: float = float("inf")
     grating_angle: float = 0.0
+    # thin-film coating (COAT_THIN_FILM, include/olb.h): layer thicknesses in micrometres (L,), the layers' n and k
+    # (L, n_wl), and the stack's incident / substrate n and k (n_wl,)
+    film_thickness: np.ndarray = field(default_factory=lambda: np.zeros(0))
+    film_n: np.ndarray = field(default_factory=lambda: np.zeros((0, 1)))
+    film_k: np.ndarray = field(default_factory=lambda: np.zeros((0, 1)))
+    film_n0: np.ndarray | None = None
+    film_k0: np.ndarray | None = None
+    film_ns: np.ndarray | None = None
+    film_ks: np.ndarray | None = None
+    # polarizer / retarder coating (COAT_POLARIZER / COAT_RETARDER): the normalised axis and the retardance in radians
+    jones_axis: np.ndarray = field(default_factory=lambda: np.array([1.0, 0.0, 0.0]))
+    retardance: float = 0.0
 
     def __post_init__(self):
         self.t = np.asarray(self.t, dtype=np.float64).reshape(3)
@@ -142,6 +168,31 @@ class SurfaceSpec:
             self.coat_n1 = np.atleast_1d(np.asarray(self.coat_n1, dtype=np.float64))
         if self.coat_n2 is not None:
             self.coat_n2 = np.atleast_1d(np.asarray(self.coat_n2, dtype=np.float64))
+        self.film_thickness = np.atleast_1d(np.asarray(self.film_thickness, dtype=np.float64)).ravel()
+        L = len(self.film_thickness)
+        self.film_n = np.asarray(self.film_n, dtype=np.float64).reshape(L, -1 if L else len(self.n1))
+        self.film_k = np.asarray(self.film_k, dtype=np.float64).reshape(L, -1 if L else len(self.n1))
+        for name in ("film_n0", "film_k0", "film_ns", "film_ks"):
+            v = getattr(self, name)
+            if v is not None:
+                setattr(self, name, np.atleast_1d(np.asarray(v, dtype=np.float64)))
+        self.jones_axis = np.asarray(self.jones_axis, dtype=np.float64).reshape(3)
+
+    def coating_block(self) -> np.ndarray:
+        """The pool block of a thin-film / polarizer / retarder coating (include/olb.h), empty for other coatings."""
+        if self.coating == COAT_THIN_FILM:
+            L, n_wl = len(self.film_thickness), len(self.n1)
+            per_wl = np.empty((n_wl, 4 + 2 * L))
+            per_wl[:, 0], per_wl[:, 1] = self.film_n0, self.film_k0
+            per_wl[:, 2], per_wl[:, 3] = self.film_ns, self.film_ks
+            per_wl[:, 4::2] = self.film_n.T
+            per_wl[:, 5::2] = self.film_k.T
+            return np.concatenate([[float(L)], self.film_thickness, per_wl.ravel()])
+        if self.coating == COAT_POLARIZER:
+            return self.jones_axis.copy()
+        if self.coating == COAT_RETARDER:
+            return np.concatenate([[self.retardance], self.jones_axis])
+        return np.zeros(0)
 
     @property
     def rotated(self) -> bool:
@@ -211,6 +262,27 @@ class SurfaceTable:
                 validate_aperture_program(s.aperture)
             if s.coating == COAT_FRESNEL and (s.coat_n1 is None or s.coat_n2 is None):
                 raise ValueError("Fresnel coating needs coat_n1/coat_n2")
+            if s.coating == COAT_THIN_FILM:
+                L = len(s.film_thickness)
+                if L > MAX_FILM_LAYERS:
+                    raise ValueError(f"thin film: {L} layers (max {MAX_FILM_LAYERS})")
+                if not np.all(np.isfinite(s.film_thickness)) or np.any(s.film_thickness < 0):
+                    raise ValueError("thin film: thicknesses must be finite and >= 0")
+                if s.film_n.shape != (L, n_wl) or s.film_k.shape != (L, n_wl):
+                    raise ValueError(f"thin film: layer indices must be ({L}, {n_wl})")
+                for name in ("film_n0", "film_k0", "film_ns", "film_ks"):
+                    v = getattr(s, name)
+                    if v is None or len(v) != n_wl:
+                        raise ValueError(f"thin film: '{name}' must have {n_wl} entries")
+                if s.kind == GEOM_NOOP:
+                    raise ValueError("thin film on an object surface")
+            elif s.coating in (COAT_POLARIZER, COAT_RETARDER):
+                if not (np.all(np.isfinite(s.jones_axis)) and np.linalg.norm(s.jones_axis) > 0):
+                    raise ValueError("polarizer / retarder: the axis must be finite and non-zero")
+                if not np.isfinite(s.retardance):
+                    raise ValueError("retarder: non-finite retardance")
+                if s.kind == GEOM_NOOP:
+                    raise ValueError("polarizer / retarder on an object surface")
             if s.interaction == INTERACT_GRATING:
                 if s.kind not in (GEOM_PLANE, GEOM_STANDARD) or (s.kind == GEOM_STANDARD and not np.isfinite(s.radius)):
                     raise ValueError("grating: only on a plane or a conic with a finite radius")
@@ -224,6 +296,11 @@ class SurfaceTable:
                     raise ValueError(f"unknown interaction {s.interaction}")
                 if nt != _PHASE_TERMS.get(s.interaction, nt) or not 1 <= nt <= MAX_PHASE_TERMS:
                     raise ValueError(f"phase profile: {nt} terms for interaction {s.interaction}")
+
+        film = sum(film_elements(len(s.film_thickness), n_wl) for s in self.surfaces if s.coating == COAT_THIN_FILM)
+        if film > MAX_FILM_ELEMENTS:
+            raise ValueError(f"thin-film stacks of this table need {film} prepared elements in shared memory "
+                             f"(more than {MAX_FILM_ELEMENTS})")
 
     @property
     def num_surfaces(self) -> int:
@@ -279,7 +356,8 @@ class SurfaceTable:
                 ints["aper_len"][j] = len(s.aperture)
             cn1 = s.coat_n1 if s.coat_n1 is not None else s.n1
             cn2 = s.coat_n2 if s.coat_n2 is not None else s.n2
-            ints["media_off"][j] = push(np.concatenate([s.n1, s.n2, s.k1, cn1, cn2]))
+            # a thin-film / polarizer / retarder block follows the media block directly (pool[media_off + 5 n_wl])
+            ints["media_off"][j] = push(np.concatenate([s.n1, s.n2, s.k1, cn1, cn2, s.coating_block()]))
             assert len(s.n1) == n_wl
             if s.interaction == INTERACT_GRATING:
                 # the phase block's framing: "efficiency" 1 (the diffractive model has none), 3 terms {m, d, alpha}
@@ -371,6 +449,18 @@ class SurfaceTable:
             m0 = int(r["media_off"])
             media = pool[m0: m0 + 5 * n_wl].reshape(5, n_wl)
             coating = int(r["coating"])
+            cb = m0 + 5 * n_wl
+            film = {}
+            if coating == COAT_THIN_FILM:
+                L = int(pool[cb])
+                per_wl = pool[cb + 1 + L: cb + 1 + L + n_wl * (4 + 2 * L)].reshape(n_wl, 4 + 2 * L)
+                film = dict(film_thickness=pool[cb + 1: cb + 1 + L].copy(), film_n=per_wl[:, 4::2].T.copy(),
+                            film_k=per_wl[:, 5::2].T.copy(), film_n0=per_wl[:, 0].copy(), film_k0=per_wl[:, 1].copy(),
+                            film_ns=per_wl[:, 2].copy(), film_ks=per_wl[:, 3].copy())
+            elif coating == COAT_POLARIZER:
+                film = dict(jones_axis=pool[cb: cb + 3].copy())
+            elif coating == COAT_RETARDER:
+                film = dict(retardance=float(pool[cb]), jones_axis=pool[cb + 1: cb + 4].copy())
             inter = int(r["interaction"])
             phase = {}
             if inter == INTERACT_GRATING:
@@ -397,6 +487,7 @@ class SurfaceTable:
                     coat_n2=media[4].copy() if coating == COAT_FRESNEL else None,
                     record=not (flags & SF_NORECORD),
                     **phase,
+                    **film,
                 )
             )
         return cls(specs, wavelengths)
