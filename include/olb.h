@@ -71,6 +71,35 @@ extern "C" {
                                       axis at distance R_rot: optiland/geometries/toroidal.py:87-232 */
 #define OLB_GEOM_FORBES_QBFS  10   /* conic + phi(r) u^2 (1 - u^2) sum a_m Q_m(u^2), u = r / norm_radius, Forbes'
                                       slope-orthogonal Q polynomials: optiland/geometries/forbes/geometry.py:187-366 */
+#define OLB_GEOM_GRID_SAG     11   /* bilinear interpolation of a table of sag values
+                                      optiland/geometries/grid_sag.py:60-140 (see "Grid sag" below) */
+#define OLB_MAX_GRID_ELEMENTS 8192 /* per table: sum over grid surfaces of nx + ny + nx * ny (e.g. 89 x 89) */
+
+/*
+ * Grid sag (GridSagGeometry).  Pool block at coef_off: x[nx], y[ny], sag[ny][nx] (row j holds y_j: sag_grid[j, i]);
+ * aux0 = nx, n_coef = ny, nx, ny >= 2, coordinates finite and strictly increasing, sag values finite.  radius is inf
+ * and conic 0; tol and max_iter are the geometry's.  The grids of one table are staged in shared memory with the rest
+ * of it, so their prepared elements (nx + ny + nx ny per surface) are capped at OLB_MAX_GRID_ELEMENTS per table.
+ * The reference's semantics, reproduced exactly:
+ *   cell      i = searchsorted(x, px, side="right") - 1 clamped to [0, nx - 2], j likewise: a point exactly on a node
+ *             takes the cell to its upper right, and the upper edge px == x[nx-1] is inside, in the last cell (the
+ *             on-axis chief ray of a grid with a node at 0 sits on that node, where the slope is discontinuous);
+ *   value     bilinear, tx = (px - x_i) / (x_{i+1} - x_i), ty likewise; the SAG is NaN outside [x_0, x_{nx-1}] x
+ *             [y_0, y_{ny-1}], the SLOPES are not: they are extrapolated from the clamped cell;
+ *   distance  Newton from t = 0 at the incoming point (no base conic): t += -f / f', f = sag - z,
+ *             f' = sx L + sy M - N (no guard on f' = 0).  An iterate that leaves the grid makes t NaN for good; a
+ *             final out-of-grid test of the intercept also gives NaN;
+ *   normal    (-sx, -sy, 1) / |.| -- the opposite sign to every other geometry's (fx, fy, -1).  Refraction and
+ *             reflection align it with the ray and do not see the sign; a phase profile on a grid substrate does.
+ * Convergence: the reference stops when the LARGEST |dt| over all rays is below tol (and, since max propagates NaN,
+ * never while some ray is NaN).  The kernel iterates each ray until its own |dt| < tol (floored at the rounding noise of
+ * t), applies that step, then takes one more (polishing) step, never more than max_iter steps in all.  Inside a cell
+ * f is a quadratic in t, so Newton converges quadratically: once |dt| < tol the remaining error is O(tol^2), and the
+ * extra steps the reference gives converged rays while others still move change t by that much at most.  A ray that
+ * never converges runs max_iter steps in both.
+ * The adjoint treats the grid values as constants: gradients flow through the pose, the indices and every other
+ * surface, not to the sag table.
+ */
 
 /* ---- OlbSurface.flags --------------------------------------------------- */
 #define OLB_SF_REFLECT     (1u << 0)  /* is_reflective: rays.reflect instead of refract
@@ -236,7 +265,7 @@ typedef struct OlbSurface {
   int32_t max_iter;    /* Newton max_iter (newton_raphson.py:58-61)           */
   int32_t coating;     /* OLB_COAT_*                                          */
   int32_t media_off;   /* pool offset of the 5 x n_wl media block             */
-  int32_t aux0;        /* polynomial: number of columns (y powers)            */
+  int32_t aux0;        /* polynomial: number of columns (y powers); grid: nx  */
   int32_t interaction; /* OLB_INTERACT_* (0: refractive / reflective)          */
   int32_t phase_off;   /* pool offset of the phase / grating block (see above) */
   double t[3];         /* effective translation                               */
@@ -495,6 +524,9 @@ int olb_trace_host_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
  * recurrence runs on (A b = a with the upper-banded f / g / h matrix of Forbes, Opt. Express 18, 19700 (2010),
  * eqs. A.14-A.16; optiland/geometries/forbes/qpoly.py:56-115), so dLoss/da = A^-T dLoss/db
  * (optiland_b200.autograd.forbes_basis_matrix).
+ * OLB_GEOM_GRID_SAG surfaces make bwd_supported 2 as well (they use none of the table blocks): the adjoint goes through
+ * the intersection with F = (sx, sy) at the hit point and through the normal with the Hessian of the bilinear cell,
+ * sxx = syy = 0, sxy = ((z22 - z21) - (z12 - z11)) / (dx dy); the grid values are constants of the adjoint.
  */
 #define OLB_GT_DIM 12
 #define OLB_GT_PER_SURFACE (2 * OLB_GT_DIM * OLB_GT_DIM)

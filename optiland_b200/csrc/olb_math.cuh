@@ -759,6 +759,74 @@ OLB_HD_CALL NewtonHit<T> newton_hit(T x, T y, T z, T L, T M, T N, const PrepSurf
   }
 }
 
+// ---- grid sag (GridSagGeometry, grid_sag.py:60-140; include/olb.h "Grid sag") ----------------------------------
+// Prepared block at S.coef_off: x[nx], y[ny], sag[ny][nx] with nx = S.poly_cols, ny = S.poly_rows.
+
+// searchsorted(c, p, side="right") - 1 clamped to [0, n - 2]: the number of nodes <= p, minus one (a NaN p counts none)
+template <typename T>
+OLB_HD int grid_cell(const T* c, int n, T p) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (c[mid] <= p) lo = mid + 1;
+    else hi = mid;
+  }
+  const int i = lo - 1;
+  return i < 0 ? 0 : (i > n - 2 ? n - 2 : i);
+}
+
+// Bilinear sag and slopes at (px, py), the reference's expressions term by term (grid_sag.py:60-100): the sag is NaN
+// outside the grid, the slopes are extrapolated from the clamped cell.  sxy (nullable): the cell's mixed derivative.
+template <typename T>
+OLB_HD T grid_eval(const PrepSurface<T>& S, const T* pool, T px, T py, T& sx, T& sy, T* sxy = nullptr) {
+  const int nx = S.poly_cols, ny = S.poly_rows;
+  const T* gx = pool + S.coef_off;
+  const T* gy = gx + nx;
+  const int i = grid_cell(gx, nx, px), j = grid_cell(gy, ny, py);
+  const T* z1 = gy + ny + j * nx + i;
+  const T z11 = z1[0], z12 = z1[1], z21 = z1[nx], z22 = z1[nx + 1];
+  const T dx = gx[i + 1] - gx[i], dy = gy[j + 1] - gy[j];
+  const T tx = o_div(px - gx[i], dx), ty = o_div(py - gy[j], dy);
+  const T ux = (T)1 - tx, uy = (T)1 - ty;
+  sx = o_div((z12 - z11) * uy + (z22 - z21) * ty, dx);
+  sy = o_div((z21 - z11) * ux + (z22 - z12) * tx, dy);
+  if (sxy) *sxy = o_div((z22 - z21) - (z12 - z11), dx * dy);
+  const bool out = px < gx[0] || px > gx[nx - 1] || py < gy[0] || py > gy[ny - 1];
+  return out ? (T)NAN : (z11 * ux + z12 * tx) * uy + (z21 * ux + z22 * tx) * ty;
+}
+
+// Intersection (GridSagGeometry.distance, grid_sag.py:108-140) and the slopes at the intercept.  Newton from t = 0;
+// each ray stops on its own |dt| < tol and takes one polishing step (include/olb.h explains why that agrees with the
+// reference's stop on the largest |dt| of all rays).  The tolerance is floored at the rounding noise of t, so that fp32
+// cannot spin to max_iter.  One copy of the interpolation serves the loop and the final out-of-grid test, which makes
+// t and the slopes NaN.
+template <typename T>
+OLB_HD NewtonHit<T> grid_hit(T x, T y, T z, T L, T M, T N, const PrepSurface<T>& S, const T* pool) {
+  NewtonHit<T> h;
+  h.status = 0;
+  T t = 0, sx = 0, sy = 0;
+  int it = 0;
+  bool polish = false, final_pass = S.max_iter <= 0;
+  for (;;) {
+    const T sag = grid_eval(S, pool, o_fma(t, L, x), o_fma(t, M, y), sx, sy);
+    if (final_pass) {
+      if (!(sag == sag)) { t = (T)NAN; sx = t; sy = t; }
+      break;
+    }
+    const T zi = o_fma(t, N, z);
+    const T dt = -o_div(sag - zi, o_fma(sx, L, o_fma(sy, M, -N)));
+    t += dt;
+    ++it;
+    T tol = S.tol;
+    const T floor_ = (T)8 * Eps<T>::v * (o_abs(t) + o_abs(zi));
+    if (floor_ > tol) tol = floor_;
+    if (polish || it >= S.max_iter || !(t == t)) final_pass = true;   // (a NaN iterate stays NaN in the reference)
+    else if (o_abs(dt) < tol) polish = true;
+  }
+  h.t = t; h.fx = sx; h.fy = sy;
+  return h;
+}
+
 // Aperture program (postfix) -> inside?   physical_apertures/*.py, see include/olb.h.
 template <typename T>
 OLB_HD bool aperture_inside(const T* prog, int len, T x, T y) {
@@ -1116,7 +1184,8 @@ OLB_HD void phase_interact(Ray<T>& r, const PrepSurface<T>& S, const T* pool, T 
 // The surface step.  FEAT gates code that most systems never need (register pressure, code
 // size); KIND (0 plane, 1 sphere/conic closed form, 2 Newton family) is resolved by the caller
 // ONCE per surface, outside the per-ray loop, so the hot loop carries no geometry branches.
-enum { KIND_PLANE = 0, KIND_CONIC = 1, KIND_NEWTON = 2, KIND_ASPHERE = 3 };   // NEWTON: any family (generic loop); ASPHERE: even / odd only (fused loop)
+enum { KIND_PLANE = 0, KIND_CONIC = 1, KIND_NEWTON = 2, KIND_ASPHERE = 3,   // NEWTON: any family (generic loop); ASPHERE: even / odd only (fused loop)
+       KIND_GRID = 4 };                                                    // grid sag (FEAT_GRID kernels only)
 
 // Ruled-grating interaction (DiffractiveInteractionModel.interact_real_rays, diffractive_model.py:28-61, with
 // RealRays.gratingdiffract): the vector form of include/olb.h (OLB_INTERACT_GRATING), which is algebraically the
@@ -1185,6 +1254,9 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
     t = -o_div(r.z, r.N);                               // plane.py:72-88
   } else if (KIND == KIND_CONIC) {
     t = conic_distance(r.x, r.y, r.z, r.L, r.M, r.N, S);
+  } else if constexpr (KIND == KIND_GRID) {
+    NewtonHit<T> h = grid_hit(r.x, r.y, r.z, r.L, r.M, r.N, S, pool);
+    t = h.t; nfx = h.fx; nfy = h.fy;
   } else {
     NewtonHit<T> h = newton_hit<T, FEAT, KIND == KIND_ASPHERE>(r.x, r.y, r.z, r.L, r.M, r.N, &S, pool);
     t = h.t; nfx = h.fx; nfy = h.fy;
@@ -1226,6 +1298,10 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
       T inv = o_rsqrt(o_fma(-S.conic * r2, c * c, (T)1));
       nx *= inv; ny *= inv; nz *= inv;
     }
+  } else if constexpr (KIND == KIND_GRID) {
+    // grid_sag.py:142-150: (-sx, -sy, 1) / |.|, the opposite sign to the other geometries (include/olb.h)
+    T inv = o_rsqrt(o_fma(nfx, nfx, o_fma(nfy, nfy, (T)1)));
+    nx = -nfx * inv; ny = -nfy * inv; nz = inv;
   } else {
     T inv = o_rsqrt(o_fma(nfx, nfx, o_fma(nfy, nfy, (T)1)));
     nx = nfx * inv; ny = nfy * inv; nz = -inv;
@@ -1297,7 +1373,11 @@ OLB_HD void surface_step(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bool
                          T* Pm = nullptr, int Pstride = 1) {
   if (S.kind == OLB_GEOM_PLANE) surface_step_k<T, FEAT, KIND_PLANE>(r, S, pool, from_global, status, Pm, Pstride);
   else if (S.kind == OLB_GEOM_STANDARD) surface_step_k<T, FEAT, KIND_CONIC>(r, S, pool, from_global, status, Pm, Pstride);
-  else if constexpr ((FEAT & FEAT_NEWTON) != 0) {
+  else if constexpr ((FEAT & FEAT_GRID) != 0) {
+    // grid-sag tables run the general kernel: the grid loop beside the one generic Newton loop
+    if (S.kind == OLB_GEOM_GRID_SAG) surface_step_k<T, FEAT, KIND_GRID>(r, S, pool, from_global, status, Pm, Pstride);
+    else surface_step_k<T, FEAT, KIND_NEWTON>(r, S, pool, from_global, status, Pm, Pstride);
+  } else if constexpr ((FEAT & FEAT_NEWTON) != 0) {
     // without FEAT_FREEFORM every Newton surface of the table is an even / odd asphere: the fused loop; with
     // it, one generic loop serves all families (two loops in one kernel cost more I-cache than the fusion saves)
     if constexpr ((FEAT & FEAT_FREEFORM) != 0) surface_step_k<T, FEAT, KIND_NEWTON>(r, S, pool, from_global, status, Pm, Pstride);
@@ -1552,6 +1632,16 @@ OLB_HD bool surface_backward(const PrepSurface<T>& S, const T* pool, T xg0, T yg
     jxx = pax * S.inv_norm * Dxx; jxy = pax * S.inv_norm_y * Dxy;
     jyx = pay * S.inv_norm * Dxy; jyy = pay * S.inv_norm_y * Dyy;
   }
+  // grid sag (POLY variant only): the bilinear cell's slopes serve the intersection and the normal; its Hessian is
+  // sxx = syy = 0, sxy.  The forward normal (-sx, -sy, 1) / |.| is the negative of the (fx, fy, -1) / |.| used here,
+  // which refraction and reflection (through the aligned normal) do not see.  The grid values are constants.
+  const bool grid = POLY && S.kind == OLB_GEOM_GRID_SAG;
+  if (grid) {
+    T sxy;
+    (void)grid_eval(S, pool, x1, y1, fx, fy, &sxy);
+    Fx = fx; Fy = fy;
+    jxy = sxy; jyx = sxy;
+  }
   const T invG = plane ? (T)1 : o_rsqrt(o_fma(fx, fx, o_fma(fy, fy, (T)1)));
   // unit normal: plane (0,0,+1) (plane.py:90-109), otherwise (fx, fy, -1)/|.|
   const T nx = plane ? (T)0 : fx * invG, ny = plane ? (T)0 : fy * invG, nz = plane ? (T)1 : -invG;
@@ -1617,10 +1707,10 @@ OLB_HD bool surface_backward(const PrepSurface<T>& S, const T* pool, T xg0, T yg
     const T ar2 = ag * gp;
     ax1 = o_fma(afx, g, (T)2 * x1 * ar2);
     ay1 = o_fma(afy, g, (T)2 * y1 * ar2);
-    if (polyfam) {
+    if (polyfam || grid) {
       ax1 += o_fma(afx, jxx, afy * jyx);
       ay1 += o_fma(afx, jxy, afy * jyy);
-      if (padj) { padj->ax = afx * pax; padj->ay = afy * pay; }
+      if (polyfam && padj) { padj->ax = afx * pax; padj->ay = afy * pay; }
     }
   }
   // ---- clip / absorption / OPD ------------------------------------------------------------------
@@ -1649,7 +1739,7 @@ OLB_HD bool surface_backward(const PrepSurface<T>& S, const T* pool, T xg0, T yg
   const T qt = q * t;
   adL = o_fma(qt, Fx, adL); adM = o_fma(qt, Fy, adM); adN -= qt;
   if (polyfam && padj) { padj->q = q; padj->xn = pxn; padj->yn = pyn; padj->active = 1; }
-  if (!plane) {
+  if (!plane && !grid) {
     const T is = o_rcp(sconic), is3 = is * is * is, ops = (T)1 + sconic;
     // d sag / d c = r2 / (s (1+s)) ; d sag / d k = c^3 r2^2 / (2 s (1+s)^2)
     // d g / d c = 1 / s^3          ; d g / d k   = c^3 r2 / (2 s^3)

@@ -36,6 +36,7 @@ enum : uint32_t {
   FEAT_GRATING = 1u << 6,  // a ruled grating (DiffractiveInteractionModel): runs the general kernel + PHASE + this
   FEAT_JONES = 1u << 7,    // a thin-film / polarizer / retarder coating (with POL): the general polarized kernel +
                            // PHASE + GRATING + this
+  FEAT_GRID = 1u << 8,     // a grid-sag surface: the general kernel (polarized: + JONES) + PHASE + GRATING + this
 };
 
 // Prepared block of a thin-film / polarizer / retarder coating: it sits right BEFORE the surface's prepared media
@@ -252,6 +253,7 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
   std::vector<std::vector<double>> pools(tab.n_surfaces);
   uint32_t features = 0;
   int prev = -1;  // previous surface with a frame (non-NOOP)
+  int64_t grid_elements = 0;
   auto in_pool = [&](int off, int len) { return off >= 0 && len >= 0 && (int64_t)off + len <= tab.pool_len; };
 
   for (int s = 0; s < tab.n_surfaces; ++s) {
@@ -263,7 +265,7 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     o.flags = in.flags & 0xffu;
     o.max_iter = in.max_iter;
     o.coating = in.coating;
-    if (in.kind < OLB_GEOM_NOOP || in.kind > OLB_GEOM_FORBES_QBFS) { res.error = "unknown geometry kind"; return res; }
+    if (in.kind < OLB_GEOM_NOOP || in.kind > OLB_GEOM_GRID_SAG) { res.error = "unknown geometry kind"; return res; }
 
     // ---- pose --------------------------------------------------------------
     if (in.kind != OLB_GEOM_NOOP) {
@@ -311,7 +313,38 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     if (in.kind == OLB_GEOM_PLANE || in.kind == OLB_GEOM_NOOP) { o.radius = INFINITY; o.curv = 0; }
     else if (std::isinf(in.radius)) { o.curv = 0; o.flags |= PSF_RADIUS_INF; }
     else { o.curv = 1.0 / in.radius; }
-    const bool newton = in.kind >= OLB_GEOM_EVEN_ASPHERE;
+    const bool newton = in.kind >= OLB_GEOM_EVEN_ASPHERE && in.kind != OLB_GEOM_GRID_SAG;
+    if (in.kind == OLB_GEOM_GRID_SAG) {
+      // x[nx], y[ny], sag[ny][nx] as they are: the kernel's cell search and interpolation are the reference's
+      const int nx = in.aux0, ny = in.n_coef;
+      if (nx < 2 || ny < 2) { res.error = "grid sag: nx and ny must be >= 2"; return res; }
+      const int64_t elems = (int64_t)nx + ny + (int64_t)nx * ny;
+      grid_elements += elems;
+      if (grid_elements > OLB_MAX_GRID_ELEMENTS) {
+        res.error = "grid sag: the grids of this table exceed " + std::to_string(OLB_MAX_GRID_ELEMENTS) +
+                    " prepared elements (they are staged in shared memory)";
+        return res;
+      }
+      if (!in_pool(in.coef_off, (int)elems)) { res.error = "grid sag block outside pool"; return res; }
+      const double* g = tab.pool + in.coef_off;
+      for (int a = 0; a < 2; ++a) {
+        const double* c = a == 0 ? g : g + nx;
+        const int n = a == 0 ? nx : ny;
+        for (int k = 0; k < n; ++k)
+          if (!std::isfinite(c[k]) || (k > 0 && !(c[k] > c[k - 1]))) {
+            res.error = "grid sag: coordinates must be finite and strictly increasing"; return res;
+          }
+      }
+      for (int64_t k = nx + ny; k < elems; ++k)
+        if (!std::isfinite(g[k])) { res.error = "grid sag: non-finite sag value"; return res; }
+      if (in.max_iter < 0) { res.error = "negative max_iter"; return res; }
+      o.radius = INFINITY; o.curv = 0; o.conic = 0; o.kp1 = 1.0;
+      o.poly_cols = nx; o.poly_rows = ny;
+      o.coef_off = (int)pool.size();
+      pool.insert(pool.end(), g, g + elems);
+      while (pool.size() % 4) pool.push_back(0);
+      features |= FEAT_GRID;
+    }
     if (newton) {
       features |= FEAT_NEWTON;
       if (in.kind != OLB_GEOM_EVEN_ASPHERE && in.kind != OLB_GEOM_ODD_ASPHERE) { res.hints |= HINT_POLY_NEWTON; features |= FEAT_FREEFORM; }
@@ -644,8 +677,10 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
                          ((o.kind == OLB_GEOM_EVEN_ASPHERE || o.kind == OLB_GEOM_ODD_ASPHERE) && o.n_coef <= 12) || polyfam;
     // Forbes Q^bfs: covered by the general (grad_tables) variant of the adjoint kernel, at most 12 terms
     const bool forbes = o.kind == OLB_GEOM_FORBES_QBFS && tab.surfaces[s].n_coef <= 12;
-    if (polyfam || forbes) res.bwd_tables = true;
-    if (!(kind_ok || forbes) || o.coating == OLB_COAT_FRESNEL || tab.n_wl != 1)
+    // grid sag: covered by the same variant (its branch lives there, so the lean variant keeps its code)
+    const bool grid = o.kind == OLB_GEOM_GRID_SAG;
+    if (polyfam || forbes || grid) res.bwd_tables = true;
+    if (!(kind_ok || forbes || grid) || o.coating == OLB_COAT_FRESNEL || tab.n_wl != 1)
       res.bwd_supported = false;
   }
   build_blob<double>(tab, pools, ps, features, res.blob_f64);
@@ -672,6 +707,10 @@ static BatchPrep prepare_batch(const OlbTable& tmpl, const double* params, int n
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].interaction != OLB_INTERACT_REFRACT) {
       out.error = "batched tables with phase-profile or grating surfaces are not built"; out.unsupported = true; return out;
+    }
+  for (int s = 0; s < S && tmpl.surfaces; ++s)
+    if (tmpl.surfaces[s].kind == OLB_GEOM_GRID_SAG) {
+      out.error = "batched tables with grid-sag surfaces are not built"; out.unsupported = true; return out;
     }
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].coating >= OLB_COAT_THIN_FILM && tmpl.surfaces[s].coating <= OLB_COAT_RETARDER) {

@@ -345,6 +345,15 @@ __global__ void __launch_bounds__(BLOCK, (MinBlocks<T, RPT, FEAT>::v)) trace_ker
         } else if (S.kind == OLB_GEOM_STANDARD) {
 #pragma unroll
           for (int k = 0; k < RPT; ++k) surface_step_k<T, FEAT, KIND_CONIC>(r[k], S, pool, fg, status, Psm, BLOCK);
+        } else if constexpr ((FEAT & FEAT_GRID) != 0) {
+          // grid-sag tables run the general kernel (FEAT_FREEFORM): the grid loop beside the one generic Newton loop
+          if (S.kind == OLB_GEOM_GRID_SAG) {
+#pragma unroll
+            for (int k = 0; k < RPT; ++k) surface_step_k<T, FEAT, KIND_GRID>(r[k], S, pool, fg, status, Psm, BLOCK);
+          } else {
+#pragma unroll
+            for (int k = 0; k < RPT; ++k) surface_step_k<T, FEAT, KIND_NEWTON>(r[k], S, pool, fg, status, Psm, BLOCK);
+          }
         } else if constexpr ((FEAT & FEAT_NEWTON) != 0) {
           // (the launcher gives Newton tables RPT <= 2, so the unrolled bodies stay inside the I-cache.)
           // Asphere-only tables (no FEAT_FREEFORM) run the fused sag + slope loop; tables with a polynomial-family
@@ -855,6 +864,8 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       // lean polarized variants for the common systems: the general kernel's code does not fit the instruction
       // cache (no_instruction was the second largest stall of the Zernike + Fresnel configuration)
       const uint32_t g = features & ~FEAT_POL;
+      if (g & FEAT_GRID)         // grid-sag surfaces: the superset below, so every coating and DOE works on a grid
+        return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES | FEAT_GRID>(a, stream);
       if (g & FEAT_JONES)        // thin-film / polarizer / retarder coatings, on any surface (DOEs and gratings too)
         return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES>(a, stream);
       if (g & FEAT_GRATING)                                                                            // gratings (+ phase)
@@ -869,7 +880,9 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
     }
   }
   // phase-profile tables: the general kernel plus the phase interaction, one ray per thread for either caller RPT;
-  // tables with a ruled grating (phase surfaces allowed beside it) add the grating interaction to that
+  // tables with a ruled grating (phase surfaces allowed beside it) add the grating interaction to that, and tables with
+  // a grid-sag surface the grid loop to both
+  if (features & FEAT_GRID) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID>(a, stream);
   if (features & FEAT_GRATING) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING>(a, stream);
   if (features & FEAT_PHASE) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE>(a, stream);
   if (features == 0) return launch_instance<T, RPT, 0u>(a, stream);

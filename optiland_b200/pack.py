@@ -72,6 +72,7 @@ class _Prefetch:
         self.surfaces = surfaces
         self.wavelengths = wavelengths
         self.keep = []          # keeps the tensors alive so that id() stays unique while the table is in use
+        self.arrays = set()     # ids of the whole arrays among them (resolved to numpy arrays, not to floats)
         import torch
 
         self._tensor = torch.Tensor
@@ -83,6 +84,11 @@ class _Prefetch:
         elif isinstance(v, (list, tuple)):
             for u in v:
                 self._add(u)
+
+    def _add_array(self, v):
+        if isinstance(v, self._tensor) and v.dtype.is_floating_point and v.numel() > 0:
+            self.keep.append(v)
+            self.arrays.add(id(v))
 
     def _walk(self):
         for surf in self.surfaces:
@@ -96,6 +102,9 @@ class _Prefetch:
             for k in ("radius", "k", "norm_x", "norm_y", "norm_radius", "Ry", "ky", "R_rot", "k_yz",
                       "grating_order", "grating_period", "groove_orientation_angle"):
                 self._add(getattr(g, k, None))
+            if _cls(g) == "GridSagGeometry":       # the node coordinates and sag values (pack_grid_sag)
+                for k in ("x_grid", "y_grid", "sag_grid"):
+                    self._add_array(getattr(g, k, None))
             for k in ("coefficients", "coeffs_poly_y"):
                 c = getattr(g, k, None)
                 if isinstance(c, (list, tuple)):
@@ -159,9 +168,17 @@ class _Prefetch:
             for ts in groups.values():
                 import torch
 
-                vals = torch.stack([t if t.ndim == 0 else t.reshape(()) for t in ts]).detach().double().cpu().numpy()
-                for t, v in zip(ts, vals):
-                    resolved[id(t)] = float(v)
+                if not any(id(t) in self.arrays for t in ts):
+                    vals = torch.stack([t if t.ndim == 0 else t.reshape(()) for t in ts]).detach().double().cpu().numpy()
+                    for t, v in zip(ts, vals):
+                        resolved[id(t)] = float(v)
+                    continue
+                flat = torch.cat([t.reshape(-1) for t in ts]).detach().double().cpu().numpy()
+                off = 0
+                for t in ts:
+                    n = t.numel()
+                    resolved[id(t)] = flat[off:off + n].reshape(t.shape) if id(t) in self.arrays else float(flat[off])
+                    off += n
             _tls.resolved = resolved
             _Prefetch.last_count = len(resolved)
         except Exception:
@@ -287,6 +304,35 @@ def pack_phase_profile(profile) -> tuple[int, np.ndarray, float]:
     return kind, np.array(terms, dtype=np.float64), _f(profile.efficiency)
 
 
+def _grid_array(v) -> np.ndarray:
+    """A grid-sag array, from the prefetched copy when there is one (``_Prefetch``)."""
+    pre = getattr(_tls, "resolved", None)
+    r = pre.get(id(v)) if pre is not None else None
+    return np.asarray(r, dtype=np.float64) if isinstance(r, np.ndarray) else _arr(v)
+
+
+def pack_grid_sag(spec: T.SurfaceSpec, g) -> None:
+    """``GridSagGeometry`` (optiland/geometries/grid_sag.py) -> ``spec``: the node coordinates, the sag table, tol and
+    max_iter.  Grids the kernel cannot stage (more than ``T.MAX_GRID_ELEMENTS`` prepared elements), axes that are not
+    strictly increasing and non-finite values decline, each with a reason."""
+    x, y, z = (_grid_array(getattr(g, k)) for k in ("x_grid", "y_grid", "sag_grid"))
+    x, y = x.reshape(-1), y.reshape(-1)
+    nx, ny = len(x), len(y)
+    if nx < 2 or ny < 2 or z.shape != (ny, nx):
+        raise UnsupportedSurface(f"grid sag of shape {z.shape} on {ny} x {nx} nodes (at least 2 x 2)")
+    if T.grid_elements(nx, ny) > T.MAX_GRID_ELEMENTS:
+        raise UnsupportedSurface(f"grid sag of {ny} x {nx} nodes: more than {T.MAX_GRID_ELEMENTS} prepared elements "
+                                 "in shared memory")
+    for name, c in (("x", x), ("y", y)):
+        if not (np.all(np.isfinite(c)) and np.all(np.diff(c) > 0)):
+            raise UnsupportedSurface(f"grid sag {name} coordinates not finite and strictly increasing")
+    if not np.all(np.isfinite(z)):
+        raise UnsupportedSurface("grid sag with non-finite sag values")
+    spec.grid_x, spec.grid_y, spec.grid_sag = x.copy(), y.copy(), z.copy()
+    spec.tol = float(g.tol)
+    spec.max_iter = int(g.max_iter)
+
+
 _GRATING_KINDS = {"PlaneGrating": T.GEOM_PLANE, "StandardGratingGeometry": T.GEOM_STANDARD}
 
 
@@ -388,6 +434,8 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     grating = None
     if gname in _GRATING_KINDS or iname == "DiffractiveInteractionModel":
         kind, grating = pack_grating(g, iname)
+    elif gname == "GridSagGeometry":
+        kind = T.GEOM_GRID_SAG
     elif gname not in _GEOM_KINDS:
         raise UnsupportedSurface(f"geometry {gname}")
     else:
@@ -409,7 +457,9 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
     if grating is not None:
         spec.interaction = T.INTERACT_GRATING
         spec.grating_order, spec.grating_period, spec.grating_angle = grating
-    if kind != T.GEOM_PLANE:
+    if kind == T.GEOM_GRID_SAG:
+        pack_grid_sag(spec, g)          # (no radius, no conic: the geometry has neither)
+    elif kind != T.GEOM_PLANE:
         spec.radius = _f(g.radius)
         spec.conic = _f(g.k)
     if kind in T.NEWTON_KINDS:

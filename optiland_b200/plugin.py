@@ -598,12 +598,14 @@ def _live_params(surfaces, table, wavelength):
             g = surf.geometry
             cs = g.cs
             if spec.kind not in (T.GEOM_PLANE, T.GEOM_STANDARD, T.GEOM_EVEN_ASPHERE, T.GEOM_ODD_ASPHERE,
-                                 T.GEOM_POLYNOMIAL, T.GEOM_ZERNIKE, T.GEOM_CHEBYSHEV, T.GEOM_FORBES_QBFS):
+                                 T.GEOM_POLYNOMIAL, T.GEOM_ZERNIKE, T.GEOM_CHEBYSHEV, T.GEOM_FORBES_QBFS, T.GEOM_GRID_SAG):
                 return None
             # normalisation radii are constants of the adjoint.  One that an optimiser drives (NormalizationRadiusVariable,
             # optimization/variable/norm_radius.py: the value written is an nn.Parameter or computed from one) needs the
             # reference's eager graph; a plain be.array leaf -- every array is one under be.grad_mode -- does not
-            for a in ("norm_radius", "norm_x", "norm_y"):
+            # the same rule for a grid's node coordinates and sag values (constants of the adjoint: olb.h has no
+            # gradient slot for them)
+            for a in ("norm_radius", "norm_x", "norm_y", "x_grid", "y_grid", "sag_grid"):
                 v = getattr(g, a, None)
                 if getattr(v, "requires_grad", False) and (v.grad_fn is not None or isinstance(v, torch.nn.Parameter)):
                     return None
@@ -638,7 +640,7 @@ def _live_params(surfaces, table, wavelength):
             else:
                 vals[GP_TX], vals[GP_TX + 1], vals[GP_TX + 2] = scalar(cs.x, like), scalar(cs.y, like), scalar(cs.z, like)
             curved = spec.kind != T.GEOM_PLANE and np.isfinite(spec.radius)
-            if spec.kind != T.GEOM_PLANE:
+            if spec.kind not in (T.GEOM_PLANE, T.GEOM_GRID_SAG):      # (a grid has no radius and no conic)
                 vals[GP_CONIC] = scalar(g.k, like)
             flat_r.append(scalar(g.radius, like) if curved else one)
             # (a catalogue glass is a constant: the packed table already holds its index at this wavelength -- asking the
@@ -724,8 +726,9 @@ def _wants_grad(backend, surfaces, rays=None) -> bool:
             continue
         cs = g.cs
         vals = [getattr(g, "radius", None), getattr(g, "k", None), cs.x, cs.y, cs.z, cs.rx, cs.ry, cs.rz]
-        # ruled-grating scalars (pack.pack_grating)
-        vals += [getattr(g, k, None) for k in ("grating_order", "grating_period", "groove_orientation_angle")]
+        # ruled-grating scalars (pack.pack_grating) and grid-sag arrays (pack.pack_grid_sag)
+        vals += [getattr(g, k, None) for k in ("grating_order", "grating_period", "groove_orientation_angle",
+                                               "x_grid", "y_grid", "sag_grid")]
         parent = getattr(cs, "reference_cs", None)
         while parent is not None:                    # nested frames: the pose depends on every level
             vals += [parent.x, parent.y, parent.z, parent.rx, parent.ry, parent.rz]

@@ -30,6 +30,14 @@ GEOM_CHEBYSHEV = 7
 GEOM_BICONIC = 8
 GEOM_TOROIDAL = 9
 GEOM_FORBES_QBFS = 10
+GEOM_GRID_SAG = 11
+# prepared grid-sag elements of one table (olb_prep.h: nx + ny + nx * ny per surface, e.g. an 89 x 89 grid).  They are
+# staged in shared memory with the rest of the table, like the thin-film records below; include/olb.h OLB_MAX_GRID_ELEMENTS
+MAX_GRID_ELEMENTS = 8192
+
+
+def grid_elements(nx: int, ny: int) -> int:
+    return nx + ny + nx * ny
 
 SF_REFLECT = 1 << 0
 SF_ROTATED = 1 << 1
@@ -153,6 +161,10 @@ class SurfaceSpec:
     # polarizer / retarder coating (COAT_POLARIZER / COAT_RETARDER): the normalised axis and the retardance in radians
     jones_axis: np.ndarray = field(default_factory=lambda: np.array([1.0, 0.0, 0.0]))
     retardance: float = 0.0
+    # grid sag (GEOM_GRID_SAG, include/olb.h): node coordinates (nx,), (ny,) and the sag values (ny, nx), row j at y_j
+    grid_x: np.ndarray = field(default_factory=lambda: np.zeros(0))
+    grid_y: np.ndarray = field(default_factory=lambda: np.zeros(0))
+    grid_sag: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
 
     def __post_init__(self):
         self.t = np.asarray(self.t, dtype=np.float64).reshape(3)
@@ -177,6 +189,9 @@ class SurfaceSpec:
             if v is not None:
                 setattr(self, name, np.atleast_1d(np.asarray(v, dtype=np.float64)))
         self.jones_axis = np.asarray(self.jones_axis, dtype=np.float64).reshape(3)
+        self.grid_x = np.asarray(self.grid_x, dtype=np.float64).ravel()
+        self.grid_y = np.asarray(self.grid_y, dtype=np.float64).ravel()
+        self.grid_sag = np.atleast_2d(np.asarray(self.grid_sag, dtype=np.float64))
 
     def coating_block(self) -> np.ndarray:
         """The pool block of a thin-film / polarizer / retarder coating (include/olb.h), empty for other coatings."""
@@ -283,6 +298,17 @@ class SurfaceTable:
                     raise ValueError("retarder: non-finite retardance")
                 if s.kind == GEOM_NOOP:
                     raise ValueError("polarizer / retarder on an object surface")
+            if s.kind == GEOM_GRID_SAG:
+                nx, ny = len(s.grid_x), len(s.grid_y)
+                if nx < 2 or ny < 2 or s.grid_sag.shape != (ny, nx):
+                    raise ValueError(f"grid sag: {nx} x-nodes and {ny} y-nodes (>= 2 each) need ({ny}, {nx}) sag values, "
+                                     f"got {s.grid_sag.shape}")
+                for name in ("grid_x", "grid_y"):
+                    c = getattr(s, name)
+                    if not (np.all(np.isfinite(c)) and np.all(np.diff(c) > 0)):
+                        raise ValueError(f"grid sag: {name} must be finite and strictly increasing")
+                if not np.all(np.isfinite(s.grid_sag)):
+                    raise ValueError("grid sag: non-finite sag value")
             if s.interaction == INTERACT_GRATING:
                 if s.kind not in (GEOM_PLANE, GEOM_STANDARD) or (s.kind == GEOM_STANDARD and not np.isfinite(s.radius)):
                     raise ValueError("grating: only on a plane or a conic with a finite radius")
@@ -301,6 +327,10 @@ class SurfaceTable:
         if film > MAX_FILM_ELEMENTS:
             raise ValueError(f"thin-film stacks of this table need {film} prepared elements in shared memory "
                              f"(more than {MAX_FILM_ELEMENTS})")
+        grid = sum(grid_elements(len(s.grid_x), len(s.grid_y)) for s in self.surfaces if s.kind == GEOM_GRID_SAG)
+        if grid > MAX_GRID_ELEMENTS:
+            raise ValueError(f"grid-sag surfaces of this table need {grid} prepared elements in shared memory "
+                             f"(more than {MAX_GRID_ELEMENTS})")
 
     @property
     def num_surfaces(self) -> int:
@@ -345,6 +375,11 @@ class SurfaceTable:
             elif s.kind == GEOM_ZERNIKE:
                 coef = coef.reshape(-1, 4)
                 ints["n_coef"][j] = coef.shape[0]
+            elif s.kind == GEOM_GRID_SAG:
+                # x[nx], y[ny], sag[ny][nx] (include/olb.h): aux0 = nx, n_coef = ny
+                coef = np.concatenate([s.grid_x, s.grid_y, s.grid_sag.ravel()])
+                ints["n_coef"][j] = len(s.grid_y)
+                ints["aux0"][j] = len(s.grid_x)
             else:
                 ints["n_coef"][j] = coef.size
             if extra_head is not None:
@@ -439,8 +474,16 @@ class SurfaceTable:
             elif kind in (GEOM_BICONIC, GEOM_TOROIDAL):
                 head = pool[off: off + 2].copy()
                 coef = pool[off + 2: off + 2 + n_coef].copy()
+            elif kind == GEOM_GRID_SAG:
+                nx = int(r["aux0"])
+                g = pool[off: off + nx + n_coef + nx * n_coef]
+                grid = dict(grid_x=g[:nx].copy(), grid_y=g[nx:nx + n_coef].copy(),
+                            grid_sag=g[nx + n_coef:].reshape(n_coef, nx).copy())
+                coef = np.zeros(0)
             else:
                 coef = pool[off: off + n_coef].copy()
+            if kind != GEOM_GRID_SAG:
+                grid = {}
             flags = int(r["flags"])
             aper = None
             if flags & SF_APERTURE:
@@ -488,6 +531,7 @@ class SurfaceTable:
                     record=not (flags & SF_NORECORD),
                     **phase,
                     **film,
+                    **grid,
                 )
             )
         return cls(specs, wavelengths)
