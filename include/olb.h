@@ -713,6 +713,56 @@ int olb_fft_psf_accumulate_f64(const double* amp, int32_t grid_size, int32_t fir
 int olb_fft_psf_accumulate_f32(const float* amp, int32_t grid_size, int32_t first, int32_t last, double div, double mul,
                                float* psf, void* stream);
 
+/*
+ * Incoherent irradiance binning (reference: IncoherentIrradiance._generate_field_data, non-differentiable branch,
+ * optiland/analysis/irradiance.py:265-353): the weighted 2-D histogram of ray positions on a detector, in one pass.
+ *
+ *   local position  the ray point (x, y, z) in the detector surface's frame:
+ *                     OLB_IRR_FRAME_TRANSLATE: x - t[0], y - t[1] subtracted in the RAY's precision, with t the values
+ *                       the frame's x / y tensors hold (an unrotated frame without a parent: bit for bit what
+ *                       CoordinateSystem.localize's translate gives);
+ *                     OLB_IRR_FRAME_AFFINE: p_loc = R^T (p - t) in fp64, with (t, R) the frame's effective transform
+ *                       (CoordinateSystem.get_effective_transform; R row-major); zero entries of R contribute nothing,
+ *                       as a rotation by a zero angle is skipped.
+ *   mask            a ray counts when i > 0 (NaN and negative power are dropped);
+ *   bin             per axis searchsorted(edges, v, side="right") - 1 with v in its own precision compared against the
+ *                   fp64 edges; v == the last edge goes into the last bin; v outside [edges[0], edges[n]], NaN and
+ *                   +-inf are dropped (np.histogram2d);
+ *   accumulate      hist[ix * ny + iy] += (double)i, in fp64 INTO `hist` (the caller zeroes it).
+ *
+ * x / y / z / i: n_rays DEVICE values of the entry point's precision.  x_edges (nx + 1) and y_edges (ny + 1) are HOST
+ * fp64 arrays, finite and strictly increasing; the entry point copies them into the caller-owned DEVICE scratch
+ * `edges` (nx + ny + 2 doubles) on `stream`.  Every argument is checked before any device call (NULL arrays, nx or
+ * ny < 1, n_rays < 0, non-finite or non-increasing edges: OLB_ERR_INVALID_ARG).  Asynchronous on `stream`.
+ */
+#define OLB_IRR_FRAME_TRANSLATE 0
+#define OLB_IRR_FRAME_AFFINE    1
+/* Accumulation: AUTO picks from nx * ny and n_rays.  SHARED: per-CTA fp64 histograms in shared memory, flushed with one
+ * atomic per non-zero bin (nx * ny <= 27648).  GLOBAL: fp64 atomics straight into `hist`.  Lanes of a warp that hit the
+ * same bin are summed before their atomic on both paths. */
+#define OLB_IRR_PATH_AUTO   0
+#define OLB_IRR_PATH_SHARED 1
+#define OLB_IRR_PATH_GLOBAL 2
+typedef struct OlbIrradiance {
+  const void* x;
+  const void* y;
+  const void* z;              /* read by OLB_IRR_FRAME_AFFINE only; may be NULL with OLB_IRR_FRAME_TRANSLATE        */
+  const void* i;
+  int64_t n_rays;
+  int32_t frame;              /* OLB_IRR_FRAME_*                                                                   */
+  int32_t nx, ny;
+  int32_t path;               /* OLB_IRR_PATH_*: 0 lets the library choose (what callers want); the others force one
+                                 accumulation path, to measure where the choice switches                           */
+  double t[3];                /* frame origin                                                                      */
+  double R[9];                /* OLB_IRR_FRAME_AFFINE: effective rotation, row-major                               */
+  const double* x_edges;      /* HOST, nx + 1                                                                      */
+  const double* y_edges;      /* HOST, ny + 1                                                                      */
+  double* edges;              /* DEVICE scratch, nx + ny + 2                                                       */
+  double* hist;               /* DEVICE, nx * ny, row ix = x bin                                                   */
+} OlbIrradiance;              /* 184 bytes                                                                         */
+int olb_irradiance_f32(const OlbIrradiance* call, void* stream);
+int olb_irradiance_f64(const OlbIrradiance* call, void* stream);
+
 /* Number of kernel launches issued by this process through the library
  * (for bench.py's gpu_launches claim). */
 int64_t olb_launch_count(void);

@@ -85,6 +85,17 @@ class OlbTraceCall(C.Structure):
                 ("status", C.c_void_p)]
 
 
+class OlbIrradiance(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("z", C.c_void_p), ("i", C.c_void_p), ("n_rays", C.c_int64),
+                ("frame", C.c_int32), ("nx", C.c_int32), ("ny", C.c_int32), ("path", C.c_int32),
+                ("t", C.c_double * 3), ("R", C.c_double * 9), ("x_edges", C.c_void_p), ("y_edges", C.c_void_p),
+                ("edges", C.c_void_p), ("hist", C.c_void_p)]
+
+
+IRR_FRAME_TRANSLATE, IRR_FRAME_AFFINE = 0, 1
+IRR_PATH_AUTO, IRR_PATH_SHARED, IRR_PATH_GLOBAL = 0, 1, 2
+
+
 class OlbDeviceTable(C.Structure):
     _fields_ = [
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64), ("magic", C.c_uint32),
@@ -121,6 +132,8 @@ SYMBOLS = {
     "olb_fft_pupil_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "olb_fft_psf_accumulate_f64": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
     "olb_fft_psf_accumulate_f32": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
+    "olb_irradiance_f32": (C.c_int, [_P(OlbIrradiance), C.c_void_p]),
+    "olb_irradiance_f64": (C.c_int, [_P(OlbIrradiance), C.c_void_p]),
     "olb_host_scratch_bytes": (C.c_int64, [C.c_int32, C.c_int64]),
     "olb_trace_host_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbPupilLaunch), _P(OlbRays),
                                      _P(OlbRays), _P(OlbRecords), C.c_int64, C.c_int64, C.c_void_p, C.c_int64,

@@ -144,7 +144,7 @@ class CudaEngine:
         self._cache: OrderedDict[bytes, object] = OrderedDict()
         self._cache_size = cache_size
         # what went through the engine, newest last: (n_surfaces, n_rays) for a plain trace, otherwise
-        # (kind, ...) with kind in {"pupil", "wavefront", "psf", "grad", "moments", "batch"} -- the answer to
+        # (kind, ...) with kind in {"pupil", "wavefront", "psf", "grad", "moments", "batch", "irradiance"} -- the answer to
         # "did my call really run on the kernel?" (tests, plugin.stats())
         self.calls: list = []
 
@@ -281,6 +281,18 @@ class CudaEngine:
         self._note("psf", int(image_x.numel()), int(pupil_x.numel()))
         return huygens_fresnel_psf(image_x, image_y, image_z, pupil_x, pupil_y, pupil_z, pupil_amp, pupil_opd,
                                    wavelength, Rp).to(image_x.dtype)
+
+    def irradiance(self, x, y, z, power, x_edges, y_edges, frame):
+        """fp64 (nx, ny) irradiance histogram of the rays in one pass (olb_irradiance_*, optiland_b200.irradiance);
+        None to decline (not 1-D CUDA tensors of one type, device and length)."""
+        from .irradiance import bin_irradiance
+
+        ts = (x, y, z, power)
+        if not all(self.accepts_tensor(t) and t.dtype == x.dtype and t.device == x.device and t.shape == x.shape
+                   for t in ts):
+            return None
+        self._note("irradiance", len(x_edges) - 1, len(y_edges) - 1, int(x.numel()))
+        return bin_irradiance(x, y, power, x_edges, y_edges, z=z, frame=frame)
 
     def fft_pupil(self, opd_waves, intensity, cell_ray, num_rays: int, grid_size: int):
         """Padded complex pupil function of one wavelength in one pass (olb_fft_pupil_*); None to decline."""
@@ -1358,6 +1370,11 @@ def install(engine=None, alias: str | None = None) -> None:
 
     saved_fft = _fftpsf.install(sys.modules[__name__], registry, be)
 
+    # incoherent irradiance maps binned on the device (analysis/irradiance.py:265-353)
+    from . import irradiance as _irradiance
+
+    saved_irr = _irradiance.install(sys.modules[__name__], registry, be)
+
     TorchSummation.grad_wanted = _grad_wanted
     TorchSummation.compute = hf_compute
     SurfaceGroup.trace = group_trace
@@ -1367,6 +1384,7 @@ def install(engine=None, alias: str | None = None) -> None:
     _state.update(installed=True, orig_group_trace=orig_group_trace, orig_surface_trace=orig_surface_trace,
                   orig_tracer_trace=orig_tracer_trace, orig_tracer_generic=orig_tracer_generic, orig_hf_compute=orig_hf_compute, orig_chief_compute=orig_chief_compute,
                   old_backend=old, alias=alias, fuse_launch=True, fuse_wavefront=True, fuse_spot=True, fuse_fft_psf=True, fuse_aimer=True, orig_trace_subset=orig_trace_subset, orig_aim=orig_aim, saved_spot=saved_spot, saved_fft=saved_fft,
+                  saved_irr=saved_irr,
                   orig_position=orig_position, fast_positions=True, memo_paraxial=True,
                   orig_paraxial=(orig_generate, orig_epl, orig_epd, orig_positions))
 
@@ -1405,6 +1423,10 @@ def uninstall() -> None:
         from . import fftpsf as _fftpsf
 
         _fftpsf.uninstall(_state["saved_fft"])
+    if _state.get("saved_irr") is not None:
+        from . import irradiance as _irradiance
+
+        _irradiance.uninstall(_state["saved_irr"])
     if _state.get("orig_position") is not None:
         from optiland.coordinate_system import CoordinateSystem
 
