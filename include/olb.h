@@ -488,7 +488,9 @@ int olb_trace_host_f64(const OlbDeviceTable* table, int32_t first, int32_t last,
  * pose (translation gradients, and for tilted poses dLoss/dR for the caller to chain to the tilt angles), any
  * aperture tree, no or simple coating, one wavelength per call (a batch that mixes wavelengths is split by the caller:
  * one table, one forward and one adjoint launch per wavelength, optiland_b200.plugin._trace_grad_per_wavelength);
- * otherwise OLB_ERR_UNSUPPORTED.  Rays that are NaN at a surface carry no gradient.
+ * otherwise OLB_ERR_UNSUPPORTED.  Rays that are NaN at a surface carry no gradient from that surface on: neither
+ * through later rows nor through that surface's own row -- also when only part of the row is NaN, as for total
+ * internal reflection (finite intercept, intensity and OPD, NaN direction); the rows in front of it still count.
  * grad_row_mask: bit r set = record row r of grad_rec may be non-zero (rows with a clear bit
  * are not read); pass ~0 when unknown.
  */

@@ -1646,6 +1646,15 @@ OLB_HD bool surface_backward(const PrepSurface<T>& S, const T* pool, T xg0, T yg
   // unit normal: plane (0,0,+1) (plane.py:90-109), otherwise (fx, fy, -1)/|.|
   const T nx = plane ? (T)0 : fx * invG, ny = plane ? (T)0 : fy * invG, nz = plane ? (T)1 : -invG;
   const T dot = o_fma(L, nx, o_fma(M, ny, N * nz));
+  // total internal reflection: the forward pass's sqrt(1 - u^2 (1 - dot^2)) is NaN, so is the direction it records
+  // (real_rays.py:163-187), while the intercept is finite.  The ray is NaN at this surface: no gradient -- the
+  // partials below are NaN too, and even a zero adjoint times them would turn every accumulator NaN.  This drops the
+  // gradient of the row's finite entries as well (intercept, intensity, OPD at this surface): the ray contributes
+  // only through the rows in front of it.
+  if (!(S.flags & OLB_SF_REFLECT) && u != (T)1 && !(o_fma(u * u, o_fma(dot, dot, (T)-1), (T)1) >= 0)) {
+    a.x = a.y = a.z = a.L = a.M = a.N = a.i = a.opd = 0;
+    return false;
+  }
 
   // ---- adjoint of globalize ---------------------------------------------------------------
   pg[GP_TX] += a.x; pg[GP_TY] += a.y; pg[GP_TZ] += a.z;    // pg1 = R p1 + t

@@ -63,10 +63,13 @@ def run_hostcheck(hc, table, rays, dtype, first=0, last=None, want_l0=False, pma
     return out, dict(zip(REC, rec)), status.value
 
 
-def run_backward(hc, table, rays, rec, grec, dtype=np.float64, tables=False):
+def run_backward(hc, table, rays, rec, grec, dtype=np.float64, tables=False, first=0, last=None):
+    """The adjoint over surfaces [first, last): ``rays`` is the state in front of surface ``first``, ``rec`` / ``grec``
+    hold rows first .. last-1 (row 0 = surface ``first``); gradients come back for every surface of the table."""
     ht = _lib.HostTable(table)
     n = rays["x"].size
     S = table.num_surfaces
+    last = S if last is None else last
     keys = ("x", "y", "z", "L", "M", "N", "i", "w", "opd")
     rin = [np.ascontiguousarray(rays.get(k, np.zeros(n)), dtype=dtype) for k in keys]
     recs = [np.ascontiguousarray(rec[k], dtype=dtype) for k in REC]
@@ -80,12 +83,12 @@ def run_backward(hc, table, rays, rec, grec, dtype=np.float64, tables=False):
     if tables:
         gtab = np.zeros((S, 2, 12, 12), dtype=np.float64)
         fn = hc.olbhc_backward_tables_f64 if dtype == np.float64 else hc.olbhc_backward_tables_f32
-        rc = fn(C.byref(ht.c), 0, S, C.c_int64(n), P9, P8(recs), P8(grecs), P8(gin), C.c_void_p(gpar.ctypes.data),
+        rc = fn(C.byref(ht.c), first, last, C.c_int64(n), P9, P8(recs), P8(grecs), P8(gin), C.c_void_p(gpar.ctypes.data),
                 C.c_void_p(gtab.ctypes.data), err, 256)
         assert rc == 0, err.value
         return dict(zip(("x", "y", "z", "L", "M", "N", "i", "opd"), gin)), gpar, gtab
     fn = hc.olbhc_backward_f64 if dtype == np.float64 else hc.olbhc_backward_f32
-    rc = fn(C.byref(ht.c), 0, S, C.c_int64(n), P9, P8(recs), P8(grecs), P8(gin), C.c_void_p(gpar.ctypes.data), err, 256)
+    rc = fn(C.byref(ht.c), first, last, C.c_int64(n), P9, P8(recs), P8(grecs), P8(gin), C.c_void_p(gpar.ctypes.data), err, 256)
     assert rc == 0, err.value
     return dict(zip(("x", "y", "z", "L", "M", "N", "i", "opd"), gin)), gpar
 

@@ -167,6 +167,16 @@ int olbhc_bwd_supported(const OlbTable* tab) {
   PrepResult pr = prepare_table(*tab);
   return pr.error.empty() && pr.bwd_supported ? 1 : 0;
 }
+// what olb_table_upload stores in OlbDeviceTable.bwd_supported (0, 1, or 2: table gradients) and .bwd_slots
+// (PrepResult.total_gslots, the per-thread accumulator slots of the backward kernel); -1 on a table error
+int olbhc_bwd_level(const OlbTable* tab) {
+  PrepResult pr = prepare_table(*tab);
+  return pr.error.empty() ? (pr.bwd_supported ? (pr.bwd_tables ? 2 : 1) : 0) : -1;
+}
+int olbhc_bwd_slots(const OlbTable* tab) {
+  PrepResult pr = prepare_table(*tab);
+  return pr.error.empty() ? pr.total_gslots : -1;
+}
 int olbhc_trace_f64(const OlbTable* tab, int first, int last, int64_t n, double** ray, double** rec, double** l0,
                     double* pmat, int* status, char* err, int err_len) {
   return run<double>(tab, first, last, n, ray, rec, l0, pmat, status, err, err_len);
