@@ -214,9 +214,27 @@ extern "C" {
 #define OLB_AP_OFFSET_RADIAL 2 /* r_max, r_min, dx, dy   (offset_radial.py)           */
 #define OLB_AP_RECT        3   /* x_min, x_max, y_min, y_max (rectangular.py)         */
 #define OLB_AP_ELLIPSE     4   /* a, b, dx, dy           (elliptical.py)              */
+#define OLB_AP_POLYGON     5   /* n, x_0, y_0 .. x_{n-1}, y_{n-1}: the only variable-length instruction
+                                  (polygon.py: PolygonAperture and FileAperture; see below)          */
 #define OLB_AP_UNION       16  /* pops 2, pushes a | b   (base.py:259-340)            */
 #define OLB_AP_INTERSECT   17  /* pops 2, pushes a & b                                */
 #define OLB_AP_DIFFERENCE  18  /* pops 2, pushes a & ~b                               */
+/*
+ * POLYGON is the reference's torch test (backend/torch_backend.py:2013-2038, path_contains_points), an even-odd ray
+ * crossing over the vertex list closed implicitly (edge e runs from vertex e to vertex (e + 1) mod n):
+ *     cond  = (vy > py) != (vy_next > py)
+ *     slope = (vx_next - vx) / (vy_next - vy)          (one division per edge, done at upload)
+ *     x_int = vx + slope * (py - vy)                   (product rounded, then the sum: no fused multiply-add)
+ *     inside = (number of edges with cond and px < x_int) is odd
+ * in that operation order and in the table's precision, so the fp64 kernel classifies every point as the reference
+ * does.  What follows from it is reproduced as it is: a point on an edge or level with a vertex is decided by the
+ * half-open rule above (the reference's NumPy backend decides such points differently; this is the torch rule); a
+ * horizontal edge never has cond true, so it never counts and its slope is never formed; a NaN px or py is outside;
+ * clockwise and self-intersecting outlines work by parity.  3 <= n, every coordinate finite, and the polygons of one
+ * table hold at most OLB_MAX_POLYGON_VERTICES vertices together (their prepared edges are staged in shared memory with
+ * the rest of the table).  The vertices are constants of the adjoint.
+ */
+#define OLB_MAX_POLYGON_VERTICES 1024 /* per table: sum of n over every POLYGON instruction */
 
 /* ---- trace flags (OlbTraceCall.flags, `flags` of olb_trace_host_*) -------- */
 #define OLB_TF_POLARIZED   (1u << 0)  /* rays carry a 3x3 complex P matrix (OlbRays.p)  */

@@ -827,8 +827,32 @@ OLB_HD NewtonHit<T> grid_hit(T x, T y, T z, T L, T M, T N, const PrepSurface<T>&
   return h;
 }
 
-// Aperture program (postfix) -> inside?   physical_apertures/*.py, see include/olb.h.
+// OLB_AP_POLYGON (include/olb.h; prepared form: olb_prep.h PG_*): the even-odd crossing count of the reference's torch
+// backend over the edge records of the point's y-bucket.  x_int = vx + slope * (py - vy) with the product rounded
+// before the sum, as the reference's separate array operations round it.
 template <typename T>
+OLB_HD bool polygon_inside(const T* pg, T x, T y) {
+  const T ymin = pg[PG_YMIN];
+  if (!(y >= ymin && y < pg[PG_YMAX])) return false;   // no edge has cond there (NaN included)
+  const T* start = pg + (int)pg[PG_OFF];
+  const int nb = (int)pg[PG_NB];
+  const int b = polygon_bucket(y, ymin, pg[PG_SCALE], nb);
+  const T* rec = start + ((nb + 1 + 3) & ~3);
+  const int e1 = (int)start[b + 1];
+  bool odd = false;
+  for (int e = (int)start[b]; e < e1; ++e) {
+    const T* r = rec + PG_REC * e;
+    const T vy = r[1];
+    const bool cond = (vy > y) != (r[2] > y);
+    const T x_int = r[0] + o_mul_nc(r[3], y - vy);
+    odd ^= cond && (x < x_int);
+  }
+  return odd;
+}
+
+// Aperture program (postfix) -> inside?   physical_apertures/*.py, see include/olb.h.  POLYGON compiles the
+// polygon instruction in (FEAT_POLYGON kernels and the general adjoint); tables with one run only those.
+template <typename T, bool POLYGON = false>
 OLB_HD bool aperture_inside(const T* prog, int len, T x, T y) {
   uint32_t stack = 0;  // bit stack, top at bit 0
   int i = 0;
@@ -852,6 +876,9 @@ OLB_HD bool aperture_inside(const T* prog, int len, T x, T y) {
       T a = prog[i + 1], b = prog[i + 2];
       v = (o_div(dx * dx, a * a) + o_div(dy * dy, b * b)) <= (T)1;
       i += 5;
+    } else if (POLYGON && op == OLB_AP_POLYGON) {
+      v = polygon_inside(prog + i, x, y);
+      i += PG_LEN;
     } else {
       bool b_ = stack & 1u, a_ = (stack >> 1) & 1u;
       stack >>= 2;
@@ -1276,7 +1303,7 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
       T r2 = o_fma(r.x, r.x, r.y * r.y);
       inside = (r2 <= pool[S.aper_off + 1]) && (r2 >= pool[S.aper_off + 2]);
     } else if (FEAT & FEAT_EXTRA) {
-      inside = aperture_inside(pool + S.aper_off, S.aper_len, r.x, r.y);
+      inside = aperture_inside<T, (FEAT & FEAT_POLYGON) != 0>(pool + S.aper_off, S.aper_len, r.x, r.y);
     } else {
       inside = true;
     }
@@ -1728,7 +1755,7 @@ OLB_HD bool surface_backward(const PrepSurface<T>& S, const T* pool, T xg0, T yg
     bool inside = true;
     if (S.flags & OLB_SF_APERTURE)
       inside = (S.flags & PSF_APER_RADIAL) ? ((r2 <= pool[S.aper_off + 1]) && (r2 >= pool[S.aper_off + 2]))
-                                           : aperture_inside(pool + S.aper_off, S.aper_len, x1, y1);
+                                           : aperture_inside<T, POLY>(pool + S.aper_off, S.aper_len, x1, y1);
     T E = 1;
     if (S.flags & OLB_SF_ABSORBING) { E = o_exp(-med[MED_ALPHA] * t); at -= ai * i0 * med[MED_ALPHA] * E * (inside ? (T)1 : (T)0); }
     ai = inside ? ai * E : (T)0;

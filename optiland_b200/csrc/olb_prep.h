@@ -37,6 +37,7 @@ enum : uint32_t {
   FEAT_JONES = 1u << 7,    // a thin-film / polarizer / retarder coating (with POL): the general polarized kernel +
                            // PHASE + GRATING + this
   FEAT_GRID = 1u << 8,     // a grid-sag surface: the general kernel (polarized: + JONES) + PHASE + GRATING + this
+  FEAT_POLYGON = 1u << 9,  // a polygon in an aperture program: the grid-sag superset + this
 };
 
 // Prepared block of a thin-film / polarizer / retarder coating: it sits right BEFORE the surface's prepared media
@@ -60,6 +61,32 @@ enum { PH_EFF = 0, PH_NT = 1, PH_P = 2 };
 // Prepared grating block (OLB_INTERACT_GRATING), from PH_P: {sin alpha, cos alpha, tan alpha, sign(d)}, then per
 // wavelength j {m lambda_j / d, n2 = material_post's index} (GR_WL + 2 j).
 enum { GR_SIN = 0, GR_COS = 1, GR_TAN = 2, GR_SGN = 3, GR_WL = 4 };
+
+// Prepared OLB_AP_POLYGON instruction, PG_LEN elements of T in the aperture program:
+//   {opcode, [PG_NB] number of y-buckets, [PG_YMIN] min vy, [PG_YMAX] max vy, [PG_SCALE] buckets per unit y,
+//    [PG_OFF] offset of the edge block from the opcode}
+// A point with py < min vy or py >= max vy (or NaN) has `cond` false on every edge: outside, no edge is read.  The edge
+// block, 16-byte aligned, is start[nb + 1] (padded to 4) and then the edge records {vx, vy, vy_next, slope}, grouped by
+// bucket: bucket b holds records start[b] .. start[b + 1] - 1, every edge whose y-span reaches it (an edge that spans
+// several buckets is repeated in each; horizontal edges, which never cross, are left out).  The bucket of a point is
+// polygon_bucket() below, the SAME function that placed the edges; it is monotone in py, so an edge with
+// lo <= py < hi lies in [bucket(lo), bucket(hi)] -- the scan of one bucket counts exactly the crossings the scan of all
+// edges would.  Outlines of up to PG_LINEAR_MAX vertices get one bucket (a plain scan, every lane of a warp reading
+// the same record); longer ones one bucket per PG_PER_BUCKET vertices, halved until the records are at most twice
+// the edges (an outline of long zigzags would otherwise repeat every edge in every bucket).
+enum { PG_NB = 1, PG_YMIN = 2, PG_YMAX = 3, PG_SCALE = 4, PG_OFF = 5, PG_LEN = 6, PG_REC = 4,
+       PG_LINEAR_MAX = 16, PG_PER_BUCKET = 4 };
+
+#if defined(__CUDACC__)
+#define OLB_PREP_HD __host__ __device__ __forceinline__
+#else
+#define OLB_PREP_HD inline
+#endif
+template <typename T>
+OLB_PREP_HD int polygon_bucket(T y, T ymin, T scale, int nb) {
+  const int b = (int)((y - ymin) * scale);   // ymin <= y <= ymax: between 0 and nb (1 + rounding)
+  return b < nb - 1 ? b : nb - 1;
+}
 
 struct PrepHeader {
   int32_t n_surf;
@@ -186,10 +213,69 @@ struct PrepResult {
   std::string error;
 };
 
+// A polygon of one surface's aperture program: where its prepared instruction sits in the surface's pool, and its
+// vertices {x_0, y_0, ...} as uploaded.  The edge block is built per precision (polygon_build), in build_blob.
+struct PolygonSource {
+  int prog_pos;
+  std::vector<double> xy;
+};
+
+// Appends the edge block of one polygon to `pool` (whose size is a multiple of 4) and fills in the instruction at
+// pool[prog_pos].  Everything is computed in T from the vertices rounded to T, in the reference's operation order.
+template <typename T>
+static void polygon_build(const std::vector<double>& xy, size_t prog_pos, std::vector<T>& pool) {
+  const int n = (int)(xy.size() / 2);
+  struct Edge { T vx, vy, vyn, slope; };
+  std::vector<Edge> edges;
+  T ymin = (T)xy[1], ymax = (T)xy[1];
+  for (int e = 0; e < n; ++e) {
+    const int j = (e + 1) % n;
+    const T vx = (T)xy[2 * e], vy = (T)xy[2 * e + 1], vxn = (T)xy[2 * j], vyn = (T)xy[2 * j + 1];
+    if (vy < ymin) ymin = vy;
+    if (vy > ymax) ymax = vy;
+    if (vy == vyn) continue;              // horizontal: (vy > py) == (vy_next > py) for every py
+    const T dx = vxn - vx, dy = vyn - vy;
+    edges.push_back({vx, vy, vyn, (T)(dx / dy)});
+  }
+  int nb = n <= PG_LINEAR_MAX ? 1 : n / PG_PER_BUCKET;
+  T scale = 0;
+  std::vector<int> b0(edges.size()), b1(edges.size());
+  for (;; nb /= 2) {
+    scale = nb > 1 ? (T)((T)nb / (T)(ymax - ymin)) : (T)0;
+    if (!std::isfinite(scale)) { nb = 1; scale = 0; }
+    size_t records = 0;
+    for (size_t e = 0; e < edges.size(); ++e) {
+      const T lo = edges[e].vy < edges[e].vyn ? edges[e].vy : edges[e].vyn;
+      const T hi = edges[e].vy < edges[e].vyn ? edges[e].vyn : edges[e].vy;
+      b0[e] = polygon_bucket(lo, ymin, scale, nb);
+      b1[e] = polygon_bucket(hi, ymin, scale, nb);
+      records += (size_t)(b1[e] - b0[e] + 1);
+    }
+    if (nb == 1 || records <= 2 * edges.size()) break;
+  }
+  const size_t block = pool.size();
+  pool[prog_pos + PG_NB] = (T)nb;
+  pool[prog_pos + PG_YMIN] = ymin;
+  pool[prog_pos + PG_YMAX] = ymax;
+  pool[prog_pos + PG_SCALE] = scale;
+  pool[prog_pos + PG_OFF] = (T)(block - prog_pos);
+  pool.resize(block + (size_t)((nb + 1 + 3) & ~3), (T)0);
+  int count = 0;
+  for (int b = 0; b < nb; ++b) {
+    pool[block + b] = (T)count;
+    for (size_t e = 0; e < edges.size(); ++e)
+      if (b0[e] <= b && b <= b1[e]) {
+        pool.push_back(edges[e].vx); pool.push_back(edges[e].vy); pool.push_back(edges[e].vyn); pool.push_back(edges[e].slope);
+        ++count;
+      }
+  }
+  pool[block + nb] = (T)count;
+}
+
 template <typename T>
 static void build_blob(const OlbTable& tab, const std::vector<std::vector<double>>& pools,
                        const std::vector<PrepSurface<double>>& ps, uint32_t features,
-                       std::vector<unsigned char>& out) {
+                       const std::vector<std::vector<PolygonSource>>& polygons, std::vector<unsigned char>& out) {
   // flatten per-surface pools into one pool, fixing offsets
   std::vector<PrepSurface<T>> surf(ps.size());
   std::vector<T> pool;
@@ -210,6 +296,7 @@ static void build_blob(const OlbTable& tab, const std::vector<std::vector<double
     b.inv_norm_y = (T)a.inv_norm_y; b.curv_y = (T)a.curv_y; b.kp1_y = (T)a.kp1_y; b.r_rot = (T)a.r_rot;
     for (double v : pools[s]) pool.push_back((T)v);
     while (pool.size() % 4) pool.push_back((T)0);
+    for (const PolygonSource& pg : polygons[s]) polygon_build<T>(pg.xy, (size_t)base + pg.prog_pos, pool);
   }
   // wavelengths at the end of the pool
   const int wl_off = (int)pool.size();
@@ -238,7 +325,7 @@ static inline int aperture_operands(int op) {
     case OLB_AP_RADIAL: return 2;
     case OLB_AP_OFFSET_RADIAL: case OLB_AP_RECT: case OLB_AP_ELLIPSE: return 4;
     case OLB_AP_UNION: case OLB_AP_INTERSECT: case OLB_AP_DIFFERENCE: return 0;
-    default: return -1;
+    default: return -1;   // (OLB_AP_POLYGON, of variable length, is handled by the program walk itself)
   }
 }
 
@@ -253,7 +340,8 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
   std::vector<std::vector<double>> pools(tab.n_surfaces);
   uint32_t features = 0;
   int prev = -1;  // previous surface with a frame (non-NOOP)
-  int64_t grid_elements = 0;
+  int64_t grid_elements = 0, polygon_vertices = 0;
+  std::vector<std::vector<PolygonSource>> polygons(tab.n_surfaces);
   auto in_pool = [&](int off, int len) { return off >= 0 && len >= 0 && (int64_t)off + len <= tab.pool_len; };
 
   for (int s = 0; s < tab.n_surfaces; ++s) {
@@ -485,18 +573,42 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     if (in.flags & OLB_SF_APERTURE) {
       if (!in_pool(in.aper_off, in.aper_len) || in.aper_len < 1) { res.error = "aperture program outside pool"; return res; }
       int i = 0, depth = 0;
+      o.aper_off = (int)pool.size();
       while (i < in.aper_len) {
         int op = (int)tab.pool[in.aper_off + i];
         int nops = aperture_operands(op);
-        if (nops < 0) { res.error = "bad aperture opcode"; return res; }
+        if (op == OLB_AP_POLYGON) {
+          // {opcode, n, x_0, y_0, ...} -> the prepared instruction (PG_*), completed per precision in build_blob
+          const double nd = i + 1 < in.aper_len ? tab.pool[in.aper_off + i + 1] : 0.0;
+          if (!(nd >= 3 && nd <= OLB_MAX_POLYGON_VERTICES && nd == (double)(int)nd)) {
+            res.error = "polygon aperture: the vertex count must be an integer in [3, " + std::to_string(OLB_MAX_POLYGON_VERTICES) + "]";
+            return res;
+          }
+          nops = 1 + 2 * (int)nd;
+          if (i + 1 + nops > in.aper_len) { res.error = "polygon aperture: vertices outside the program"; return res; }
+          polygon_vertices += (int)nd;
+          if (polygon_vertices > OLB_MAX_POLYGON_VERTICES) {
+            res.error = "polygon aperture: the polygons of this table have more than " + std::to_string(OLB_MAX_POLYGON_VERTICES) +
+                        " vertices (their edges are staged in shared memory)";
+            return res;
+          }
+          const double* xy = tab.pool + in.aper_off + i + 2;
+          for (int k = 0; k < 2 * (int)nd; ++k)
+            if (!std::isfinite(xy[k])) { res.error = "polygon aperture: non-finite vertex"; return res; }
+          polygons[s].push_back({(int)pool.size(), std::vector<double>(xy, xy + 2 * (int)nd)});
+          pool.push_back((double)op);
+          pool.insert(pool.end(), PG_LEN - 1, 0.0);
+          features |= FEAT_POLYGON;
+        } else {
+          if (nops < 0) { res.error = "bad aperture opcode"; return res; }
+          for (int k = 0; k <= nops; ++k) pool.push_back(i + k < in.aper_len ? tab.pool[in.aper_off + i + k] : 0.0);
+        }
         if (op >= OLB_AP_UNION) { if (depth < 2) { res.error = "aperture stack underflow"; return res; } depth -= 1; }
         else { depth += 1; if (depth > 8) { res.error = "aperture program too deep"; return res; } }
         i += 1 + nops;
       }
       if (i != in.aper_len || depth != 1) { res.error = "malformed aperture program"; return res; }
-      o.aper_off = (int)pool.size();
-      o.aper_len = in.aper_len;
-      for (int k = 0; k < in.aper_len; ++k) pool.push_back(tab.pool[in.aper_off + k]);
+      o.aper_len = (int)pool.size() - o.aper_off;
       while (pool.size() % 4) pool.push_back(0);
       if ((int)tab.pool[in.aper_off] == OLB_AP_RADIAL && in.aper_len == 3) {
         o.flags |= PSF_APER_RADIAL;
@@ -680,11 +792,12 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     // grid sag: covered by the same variant (its branch lives there, so the lean variant keeps its code)
     const bool grid = o.kind == OLB_GEOM_GRID_SAG;
     if (polyfam || forbes || grid) res.bwd_tables = true;
+    if (features & FEAT_POLYGON) res.bwd_tables = true;   // the polygon scan lives in that variant too
     if (!(kind_ok || forbes || grid) || o.coating == OLB_COAT_FRESNEL || tab.n_wl != 1)
       res.bwd_supported = false;
   }
-  build_blob<double>(tab, pools, ps, features, res.blob_f64);
-  build_blob<float>(tab, pools, ps, features, res.blob_f32);
+  build_blob<double>(tab, pools, ps, features, polygons, res.blob_f64);
+  build_blob<float>(tab, pools, ps, features, polygons, res.blob_f32);
   return res;
 }
 

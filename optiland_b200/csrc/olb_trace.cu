@@ -864,6 +864,8 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       // lean polarized variants for the common systems: the general kernel's code does not fit the instruction
       // cache (no_instruction was the second largest stall of the Zernike + Fresnel configuration)
       const uint32_t g = features & ~FEAT_POL;
+      if (g & FEAT_POLYGON)      // polygon apertures: the grid-sag superset + the polygon scan, so a polygon works on any surface
+        return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES | FEAT_GRID | FEAT_POLYGON>(a, stream);
       if (g & FEAT_GRID)         // grid-sag surfaces: the superset below, so every coating and DOE works on a grid
         return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES | FEAT_GRID>(a, stream);
       if (g & FEAT_JONES)        // thin-film / polarizer / retarder coatings, on any surface (DOEs and gratings too)
@@ -881,7 +883,9 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
   }
   // phase-profile tables: the general kernel plus the phase interaction, one ray per thread for either caller RPT;
   // tables with a ruled grating (phase surfaces allowed beside it) add the grating interaction to that, and tables with
-  // a grid-sag surface the grid loop to both
+  // a grid-sag surface the grid loop to both; tables with a polygon aperture the polygon scan to all three
+  if (features & FEAT_POLYGON)
+    return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON>(a, stream);
   if (features & FEAT_GRID) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID>(a, stream);
   if (features & FEAT_GRATING) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING>(a, stream);
   if (features & FEAT_PHASE) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE>(a, stream);

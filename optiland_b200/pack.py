@@ -125,6 +125,8 @@ class _Prefetch:
                 a = stack.pop()
                 for k in ("r_max", "r_min", "offset_x", "offset_y", "x_min", "x_max", "y_min", "y_max"):
                     self._add(getattr(a, k, None))
+                if _cls(a) in ("PolygonAperture", "FileAperture"):      # the vertex array (pack_aperture)
+                    self._add_array(getattr(a, "vertices", None))
                 for k in ("a", "b"):
                     u = getattr(a, k, None)
                     if u is not None and hasattr(u, "contains"):
@@ -220,6 +222,17 @@ def pack_aperture(ap) -> np.ndarray:
            "DifferenceAperture": T.AP_DIFFERENCE}
     if name in ops:
         return T.aperture_combine(ops[name], pack_aperture(ap.a), pack_aperture(ap.b))
+    if name in ("PolygonAperture", "FileAperture"):
+        # the exact classes only (a subclass may override contains); the LIVE vertices, which scale() rewrites
+        v = _grid_array(ap.vertices)
+        if v.ndim != 2 or v.shape[1] != 2 or v.shape[0] < 3:
+            raise UnsupportedSurface(f"polygon aperture with vertices of shape {v.shape} (at least 3 x 2)")
+        if v.shape[0] > T.MAX_POLYGON_VERTICES:
+            raise UnsupportedSurface(f"polygon aperture of {v.shape[0]} vertices: more than {T.MAX_POLYGON_VERTICES} "
+                                     "prepared in shared memory")
+        if not np.all(np.isfinite(v)):
+            raise UnsupportedSurface("polygon aperture with non-finite vertices")
+        return T.aperture_polygon(v[:, 0], v[:, 1])
     raise UnsupportedSurface(f"aperture type {name}")
 
 
@@ -305,7 +318,7 @@ def pack_phase_profile(profile) -> tuple[int, np.ndarray, float]:
 
 
 def _grid_array(v) -> np.ndarray:
-    """A grid-sag array, from the prefetched copy when there is one (``_Prefetch``)."""
+    """A grid-sag or polygon-vertex array, from the prefetched copy when there is one (``_Prefetch``)."""
     pre = getattr(_tls, "resolved", None)
     r = pre.get(id(v)) if pre is not None else None
     return np.asarray(r, dtype=np.float64) if isinstance(r, np.ndarray) else _arr(v)
@@ -544,7 +557,12 @@ def pack_surface_group(surface_group, wavelengths) -> T.SurfaceTable:
     if len(surfaces) > T.MAX_SURFACES:
         raise UnsupportedSurface(f"more than {T.MAX_SURFACES} surfaces")
     with _Prefetch(surfaces, wavelengths):
-        return T.SurfaceTable([pack_surface(s, wavelengths) for s in surfaces], wavelengths)
+        specs = [pack_surface(s, wavelengths) for s in surfaces]
+        nv = sum(T.polygon_vertices(s.aperture) for s in specs if s.aperture is not None)
+        if nv > T.MAX_POLYGON_VERTICES:
+            raise UnsupportedSurface(f"polygon apertures with {nv} vertices in all: more than {T.MAX_POLYGON_VERTICES} "
+                                     "prepared in shared memory")
+        return T.SurfaceTable(specs, wavelengths)
 
 
 def launch_scalars(optic, Hx: float, Hy: float) -> dict:

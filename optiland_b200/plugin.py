@@ -617,10 +617,16 @@ def _live_params(surfaces, table, wavelength):
             # reference's eager graph; a plain be.array leaf -- every array is one under be.grad_mode -- does not
             # the same rule for a grid's node coordinates and sag values (constants of the adjoint: olb.h has no
             # gradient slot for them)
+            # and for the vertices of polygon apertures (the clip mask is a constant of the adjoint)
             for a in ("norm_radius", "norm_x", "norm_y", "x_grid", "y_grid", "sag_grid"):
                 v = getattr(g, a, None)
                 if getattr(v, "requires_grad", False) and (v.grad_fn is not None or isinstance(v, torch.nn.Parameter)):
                     return None
+            # the vertices of polygon apertures are constants too (the clip mask has no gradient).  PolygonAperture
+            # always COMPUTES them (column_stack of x and y; scale() multiplies them), so under be.grad_mode they carry
+            # a grad_fn without anybody driving them: what declines is an nn.Parameter among the leaves of their graph
+            if any(_parameter_driven(v) for v in _polygon_vertices(surf)):
+                return None
             nested = cs.reference_cs is not None
             if nested:
                 # a frame defined relative to another one (coordinate breaks of imported systems,
@@ -681,6 +687,37 @@ def _live_params(surfaces, table, wavelength):
     radius = torch.stack(flat_r)
     curv = P[:, GP_CURV] / radius
     return torch.cat([P[:, :GP_CURV], curv[:, None], P[:, GP_CURV + 1:]], dim=1)
+
+
+def _polygon_vertices(surf) -> list:
+    """The vertex arrays of every polygon in the surface's aperture tree (pack.pack_aperture)."""
+    out, stack = [], [getattr(surf, "aperture", None)]
+    while stack:
+        a = stack.pop()
+        if a is None:
+            continue
+        if type(a).__name__ in ("PolygonAperture", "FileAperture"):
+            out.append(getattr(a, "vertices", None))
+        stack += [u for u in (getattr(a, "a", None), getattr(a, "b", None)) if hasattr(u, "contains")]
+    return out
+
+
+def _parameter_driven(v) -> bool:
+    """True when ``v`` is an nn.Parameter or is computed from one."""
+    import torch
+
+    if isinstance(v, torch.nn.Parameter):
+        return True
+    seen, stack = set(), [getattr(v, "grad_fn", None)]
+    while stack:
+        fn = stack.pop()
+        if fn is None or fn in seen:
+            continue
+        seen.add(fn)
+        if isinstance(getattr(fn, "variable", None), torch.nn.Parameter):
+            return True
+        stack += [f for f, _ in fn.next_functions]
+    return False
 
 
 def _live_coefs(surfaces, table):
@@ -757,6 +794,7 @@ def _wants_grad(backend, surfaces, rays=None) -> bool:
             pc = getattr(pp, "coefficients", None)
             if pc is not None:
                 vals += [pc] if hasattr(pc, "requires_grad") else list(np.ravel(np.asarray(pc, dtype=object)))
+        vals += _polygon_vertices(surf)              # polygon apertures (pack.pack_aperture)
         jones = getattr(getattr(getattr(surf, "interaction_model", None), "coating", None), "jones", None)
         if jones is not None:                        # thin-film thicknesses, retardance (pack.pack_jones_coating)
             vals += [getattr(layer, "thickness_um", None) for layer in getattr(getattr(jones, "stack", None), "layers", [])]

@@ -75,6 +75,10 @@ AP_RADIAL = 1
 AP_OFFSET_RADIAL = 2
 AP_RECT = 3
 AP_ELLIPSE = 4
+AP_POLYGON = 5      # the only variable-length instruction: n, then the n (x, y) pairs (include/olb.h)
+# vertices of all the polygons of one table: their prepared edges are staged in shared memory with the rest of the table
+# (include/olb.h OLB_MAX_POLYGON_VERTICES)
+MAX_POLYGON_VERTICES = 1024
 AP_UNION = 16
 AP_INTERSECT = 17
 AP_DIFFERENCE = 18
@@ -233,15 +237,39 @@ class SurfaceSpec:
         return f
 
 
+def _polygon_operands(prog: np.ndarray, i: int) -> int:
+    """Operand count of the AP_POLYGON instruction at ``prog[i]``: the vertex count and the n (x, y) pairs."""
+    nv = prog[i + 1] if i + 1 < len(prog) else 0.0
+    if not (nv >= 3 and nv == int(nv)):
+        raise ValueError(f"polygon aperture: the vertex count must be an integer >= 3, got {nv!r}")
+    nv = int(nv)
+    if i + 2 + 2 * nv > len(prog):
+        raise ValueError("polygon aperture: vertices outside the program")
+    if not np.all(np.isfinite(prog[i + 2: i + 2 + 2 * nv])):
+        raise ValueError("polygon aperture: non-finite vertex")
+    return 1 + 2 * nv
+
+
+def polygon_vertices(prog: np.ndarray) -> int:
+    """Vertices of all the polygons of a (valid) aperture program."""
+    i, total = 0, 0
+    while i < len(prog):
+        op = int(prog[i])
+        nops = _polygon_operands(prog, i) if op == AP_POLYGON else _AP_OPERANDS[op]
+        total += (nops - 1) // 2 if op == AP_POLYGON else 0
+        i += 1 + nops
+    return total
+
+
 def validate_aperture_program(prog: np.ndarray) -> None:
     """Check a postfix aperture program is well formed (stack depth ends at 1)."""
     i, depth = 0, 0
     n = len(prog)
     while i < n:
-        op = int(prog[i])
-        if op not in _AP_OPERANDS or prog[i] != op:
+        op = int(prog[i]) if np.isfinite(prog[i]) else -1
+        if (op not in _AP_OPERANDS and op != AP_POLYGON) or prog[i] != op:
             raise ValueError(f"bad aperture opcode {prog[i]!r} at {i}")
-        nops = _AP_OPERANDS[op]
+        nops = _polygon_operands(prog, i) if op == AP_POLYGON else _AP_OPERANDS[op]
         if op >= AP_UNION:
             if depth < 2:
                 raise ValueError("aperture program stack underflow")
@@ -327,6 +355,10 @@ class SurfaceTable:
         if film > MAX_FILM_ELEMENTS:
             raise ValueError(f"thin-film stacks of this table need {film} prepared elements in shared memory "
                              f"(more than {MAX_FILM_ELEMENTS})")
+        nv = sum(polygon_vertices(s.aperture) for s in self.surfaces if s.aperture is not None)
+        if nv > MAX_POLYGON_VERTICES:
+            raise ValueError(f"polygon apertures of this table have {nv} vertices: their prepared edges are staged in "
+                             f"shared memory (at most {MAX_POLYGON_VERTICES})")
         grid = sum(grid_elements(len(s.grid_x), len(s.grid_y)) for s in self.surfaces if s.kind == GEOM_GRID_SAG)
         if grid > MAX_GRID_ELEMENTS:
             raise ValueError(f"grid-sag surfaces of this table need {grid} prepared elements in shared memory "
@@ -558,6 +590,12 @@ def aperture_rect(x_min, x_max, y_min, y_max) -> np.ndarray:
 
 def aperture_ellipse(a, b, dx=0.0, dy=0.0) -> np.ndarray:
     return np.array([AP_ELLIPSE, a, b, dx, dy], dtype=np.float64)
+
+
+def aperture_polygon(x, y) -> np.ndarray:
+    """Vertices (x_k, y_k) of a polygon, closed implicitly; any orientation, self-intersections allowed (even-odd)."""
+    xy = np.stack([np.asarray(x, dtype=np.float64).ravel(), np.asarray(y, dtype=np.float64).ravel()], axis=1)
+    return np.concatenate([[AP_POLYGON, float(len(xy))], xy.ravel()])
 
 
 def aperture_combine(op: int, a: Sequence[float], b: Sequence[float]) -> np.ndarray:
