@@ -489,13 +489,22 @@ class SurfaceGroup:
         return rays
 
     def spot_moments(self, rays=None, pupil=None, center=(0.0, 0.0), dtype=None):
-        """Fused trace + spot/OPD moments (no per-ray output at all); see ``trace_moments_device``."""
+        """Fused trace + spot/OPD moments (no per-ray output at all); see ``trace_moments_device``.
+
+        ``rms_centroid`` comes from a second launch whose moments are taken about the first one's centroid: the
+        one-pass ``m3/n - mx^2 - my^2`` about ``center`` cancels the spot's offset from it (a micrometre spot 20 mm off
+        axis keeps only a few digits), as ``spot.py`` avoids for SpotDiagram."""
         if pupil is not None:
             n, dt = pupil[0].numel(), pupil[0].dtype
         else:
             n, dt = len(rays), rays.dtype
         m = trace_moments_device(self.device_table, n, dtype or dt, rays=rays, pupil=pupil, center=center)
-        return moments_to_spot(m, center)
+        out = moments_to_spot(m, center)
+        cen = out.get("centroid")
+        if cen is not None and np.isfinite(cen[0]) and np.isfinite(cen[1]):
+            m2 = trace_moments_device(self.device_table, n, dtype or dt, rays=rays, pupil=pupil, center=cen)
+            out["rms_centroid"] = moments_to_spot(m2, cen)["rms_centroid"]
+        return out
 
     def _get(self, key):
         if self._rec is None:
