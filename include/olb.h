@@ -109,6 +109,42 @@ extern "C" {
 #define OLB_SF_ABSORBING   (1u << 3)  /* some k1(lambda) > 0: Beer-Lambert attenuation
                                          optiland/propagation/homogeneous.py:45-53            */
 #define OLB_SF_NORECORD    (1u << 4)  /* do not write this surface's record row              */
+#define OLB_SF_BSDF        (1u << 5)  /* interaction_model.bsdf is set: scatter after the interaction (see below) */
+
+/* ---- BSDF scatter (OLB_SF_BSDF) ------------------------------------------
+ * LambertianBSDF / GaussianBSDF (optiland/scatter.py) on any surface of an unpolarized trace.  Block at
+ * pool[media_off + 5 * n_wl] (a thin-film / polarizer / retarder block then follows it):
+ *   {kind, sigma, seed_lo, seed_hi}   kind OLB_BSDF_*, sigma finite (read by GAUSSIAN only), the seed halves integers
+ *                                     in [0, 2^32): the Philox key of this surface.
+ * Order per surface (interactions/base.py:111-128): intersect, OPD, clip (clipped rays, i = 0, are scattered too),
+ * interact (refract / reflect, phase profile or ruled grating), SCATTER, coating.  The scatter takes the interaction's
+ * outgoing direction r = (L, M, N) and the geometry's normal n AS surface_normal RETURNS IT -- not aligned with the ray:
+ * (0, 0, 1) on a plane, pointing to -z on conics and the Newton families, to +z on a grid sag -- and does:
+ *     arb = (1, 0, 0) if L < 0.999 else (0, 1, 0)        (tested on the ray's L, not on n)
+ *     a = normalise(n x arb);  b = n x a                  (b is not re-normalised)
+ *     repeat: (x, y) = draw(attempt);  sx = r.a + x;  sy = r.b + y;  rad = 1 - sx^2 - sy^2   until not (rad < 0)
+ *     d := sx a + sy b + sqrt(rad) n                      (not re-normalised)
+ * with draw LAMBERTIAN: u, v uniform in [0, 1):  (sqrt(u) cos 2 pi v, sqrt(u) sin 2 pi v)
+ *           GAUSSIAN:   u1 uniform in (0, 1], u2 in [0, 1):  sigma sqrt(-2 log u1) (cos 2 pi u2, sin 2 pi u2)
+ * The reference's behaviours are reproduced as they are:
+ *   1. a transmissive surface scatters into the hemisphere of n: BACKWARDS on a conic (N ~ -1 after a lens surface),
+ *      forwards on a plane and a grid sag;
+ *   2. a normal parallel to x while L < 0.999 makes a = 0 / 0: the ray leaves with a NaN direction;
+ *   3. a NaN rad ends the loop: NaN rays stay NaN after one draw and never loop.
+ * Random numbers: cuRAND's stateless Philox4x32-10 (Salmon et al., SC11), one call per attempt:
+ *     key = (seed_lo, seed_hi),  counter = (ray & 0xffffffff, ray >> 32, rng_stream, attempt)
+ * where `ray` is the ray's index in the call's arrays (olb_trace_host_*: in the whole host array, stream 0) and
+ * rng_stream is OlbTraceCall.rng_stream.  Its four words make two 53-bit uniforms, u = (w0 >> 5, w1 >> 6) / 2^53 and
+ * v from (w2, w3) alike (u1 = u + 2^-53, in (0, 1]), which are then rounded to the kernel's type, so both precisions
+ * draw the same numbers and a ray's draws do not depend on the kernel variant, the grid or the host path's chunking.
+ * The reference loops without a bound; an absurd sigma makes its acceptance rate about 1 / (2 sigma^2).  The kernel
+ * stops after OLB_BSDF_MAX_ATTEMPTS draws: the ray leaves with a NaN direction and OLB_ST_BSDF_ATTEMPTS is set.
+ * A table with a BSDF has bwd_supported = 0, olb_table_upload_batch rejects it, and a polarized trace of it
+ * (OLB_TF_POLARIZED, or a Fresnel / thin-film / polarizer / retarder coating) is OLB_ERR_UNSUPPORTED.
+ */
+#define OLB_BSDF_LAMBERTIAN 1
+#define OLB_BSDF_GAUSSIAN   2
+#define OLB_BSDF_MAX_ATTEMPTS 65536
 
 /* ---- coatings (OlbSurface.coating) -------------------------------------- */
 #define OLB_COAT_NONE      0   /* rays.update() : identity for RealRays, basis change
@@ -271,7 +307,8 @@ extern "C" {
  *     pool[media_off + 4*n_wl + j] = coating n2 (FresnelCoating.material_post)
  * evaluated on the host by the reference's own material classes
  * (optiland/materials/base.py:98-149).  A thin-film, polarizer or retarder coating's block follows at
- * pool[media_off + 5*n_wl] (see OLB_COAT_THIN_FILM).
+ * pool[media_off + 5*n_wl] (see OLB_COAT_THIN_FILM), or at pool[media_off + 5*n_wl + 4] behind a BSDF block
+ * (OLB_SF_BSDF).
  */
 typedef struct OlbSurface {
   int32_t kind;        /* OLB_GEOM_*                                          */
@@ -373,6 +410,8 @@ typedef struct OlbRecords {
 
 #define OLB_ST_K_PARALLEL_X (1 << 2)    /* polarized intensity epilogue: a launch direction parallel to the x axis; the
                                           reference raises ValueError (optiland/rays/polarized_rays.py:216-218)     */
+#define OLB_ST_BSDF_ATTEMPTS (1 << 3)   /* a BSDF scatter drew OLB_BSDF_MAX_ATTEMPTS rejected directions; that ray's
+                                          direction is NaN (the reference would loop for ever, scatter.py)        */
 
 int olb_version(void);
 /* Copies the calling thread's last error message into buf (NUL terminated). */
@@ -653,7 +692,8 @@ typedef struct OlbTraceCall {
   int32_t first, last;
   int64_t n_rays;
   uint32_t flags;             /* OLB_TF_*                                                                        */
-  int32_t reserved;
+  uint32_t rng_stream;        /* Philox counter word of BSDF scatter draws (OLB_SF_BSDF); read by BSDF tables only.
+                                 A caller that wants independent draws on every call advances it per call.     */
   /* Device SoA (updated in place unless OLB_TF_NO_FINAL).  With `launch` it receives the final state
    * (x,y,z,L,M,N,i,opd; not needed with OLB_TF_NO_FINAL) and supplies `w` when the table has several wavelengths;
    * then, and whenever nothing would be read or written, it may be NULL. */

@@ -78,7 +78,7 @@ class OlbPolarization(C.Structure):
 
 class OlbTraceCall(C.Structure):
     _fields_ = [("first", C.c_int32), ("last", C.c_int32), ("n_rays", C.c_int64), ("flags", C.c_uint32),
-                ("reserved", C.c_int32), ("rays", C.POINTER(OlbRays)), ("rec", C.POINTER(OlbRecords)),
+                ("rng_stream", C.c_uint32), ("rays", C.POINTER(OlbRays)), ("rec", C.POINTER(OlbRecords)),
                 ("launch", C.POINTER(OlbPupilLaunch)), ("center", C.c_double * 2), ("moments", C.c_void_p),
                 ("rays_per_system", C.c_int64), ("wavefront_ref", C.POINTER(OlbWavefrontRef)),
                 ("wavefront_out", C.POINTER(OlbWavefrontOut)), ("pol", C.POINTER(OlbPolarization)),

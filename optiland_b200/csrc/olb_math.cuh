@@ -87,6 +87,8 @@ struct Ray {
   T opd_lo;    // fp32 only: low word of a two-float OPD accumulator (see accumulate_opd)
   T L0, M0, N0;  // direction before the last interaction (real_rays.py:170-172)
   int widx;    // wavelength index into the media tables
+  uint64_t id;      // FEAT_BSDF only: the ray's index, counter of its scatter draws (olb_bsdf.cuh)
+  uint32_t stream;  //                 and the call's rng_stream
   T P[18];     // FEAT_POL only: 3x3 complex polarization matrix, P[2*(3r+c)] = Re, +1 = Im
                // (optiland/rays/polarized_rays.py:50); untouched (and optimised away) otherwise
 };
@@ -1260,6 +1262,10 @@ OLB_HD void grating_interact(Ray<T>& r, const PrepSurface<T>& S, const T* pool, 
   r.N = kz * inv;
 }
 
+// BSDF scatter (include/olb.h OLB_SF_BSDF), defined in olb_bsdf.cuh: compiled only into FEAT_BSDF kernels.
+template <typename T>
+OLB_HD void bsdf_scatter(Ray<T>& r, const T* bs, T nx, T ny, T nz, int& status);
+
 template <typename T, uint32_t FEAT, int KIND>
 OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bool from_global, int& status,
                            T* Pm = nullptr, int Pstride = 1) {
@@ -1373,6 +1379,10 @@ OLB_HD void surface_step_k(Ray<T>& r, const PrepSurface<T>& S, const T* pool, bo
     r.L = o_fma(u, r.L, nx * g);
     r.M = o_fma(u, r.M, ny * g);
     r.N = o_fma(u, r.N, nz * g);
+  }
+  // -- scatter (interactions/base.py:115-116): about the outgoing direction, with the unaligned normal
+  if constexpr ((FEAT & FEAT_BSDF) != 0) {
+    if (S.flags & OLB_SF_BSDF) bsdf_scatter(r, pool + S.media_off - BS_LEN, nx, ny, nz, status);
   }
   // -- coating (interactions/base.py:111-128; coatings.py:164-237)
   if ((FEAT & FEAT_EXTRA) && S.coating == OLB_COAT_SIMPLE)

@@ -38,7 +38,14 @@ enum : uint32_t {
                            // PHASE + GRATING + this
   FEAT_GRID = 1u << 8,     // a grid-sag surface: the general kernel (polarized: + JONES) + PHASE + GRATING + this
   FEAT_POLYGON = 1u << 9,  // a polygon in an aperture program: the grid-sag superset + this
+  FEAT_BSDF = 1u << 10,    // a BSDF scatter (OLB_SF_BSDF): the polygon superset + this (unpolarized only)
 };
+
+// Prepared BSDF block of a surface with OLB_SF_BSDF: BS_LEN elements of T right BEFORE its prepared media block (the
+// kernel finds it from PrepSurface::media_off alone; a BSDF table never runs the polarized kernels, whose coating
+// header sits there instead): {kind, sigma, key bits 0-15, 16-31, 32-47, 48-63, 0, 0}.  The 64-bit Philox key is kept
+// in 16-bit pieces, each exact in fp32, so both precisions draw with the same key.
+enum { BS_KIND = 0, BS_SIGMA = 1, BS_KEY = 2, BS_LEN = 8 };
 
 // Prepared block of a thin-film / polarizer / retarder coating: it sits right BEFORE the surface's prepared media
 // block, so the kernel finds it from PrepSurface::media_off alone.  Its CO_HDR-element header ends at media_off:
@@ -624,10 +631,32 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     // ---- media -----------------------------------------------------------------
     if (!in_pool(in.media_off, 5 * n_wl)) { res.error = "media block outside pool"; return res; }
 
+    // ---- BSDF block {kind, sigma, seed_lo, seed_hi} at media_off + 5 n_wl (include/olb.h) -----------------------
+    const bool bsdf = (in.flags & OLB_SF_BSDF) != 0;
+    double bsdf_block[BS_LEN] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (bsdf) {
+      if (in.kind == OLB_GEOM_NOOP) { res.error = "BSDF on an object surface"; return res; }
+      const int bb = in.media_off + 5 * n_wl;
+      if (!in_pool(bb, 4)) { res.error = "BSDF block outside pool"; return res; }
+      const double* b = tab.pool + bb;
+      if (b[0] != OLB_BSDF_LAMBERTIAN && b[0] != OLB_BSDF_GAUSSIAN) { res.error = "bad BSDF block: unknown kind"; return res; }
+      if (!std::isfinite(b[1])) { res.error = "bad BSDF block: non-finite sigma"; return res; }
+      for (int q = 2; q < 4; ++q)
+        if (!(b[q] >= 0 && b[q] < 4294967296.0 && b[q] == std::floor(b[q]))) {
+          res.error = "bad BSDF block: the seed halves must be integers in [0, 2^32)"; return res;
+        }
+      const uint64_t key = (uint64_t)b[2] | ((uint64_t)b[3] << 32);
+      bsdf_block[BS_KIND] = b[0];
+      bsdf_block[BS_SIGMA] = b[1];
+      for (int q = 0; q < 4; ++q) bsdf_block[BS_KEY + q] = (double)((key >> (16 * q)) & 0xffffu);
+      features |= FEAT_BSDF;
+      res.bwd_supported = false;       // the adjoint has no scatter
+    }
+
     // ---- thin-film / polarizer / retarder coating: its prepared block goes right before the media block ------
     if (in.coating >= OLB_COAT_THIN_FILM && in.coating <= OLB_COAT_RETARDER) {
       if (in.kind == OLB_GEOM_NOOP) { res.error = "polarizing coating on an object surface"; return res; }
-      const int cb = in.media_off + 5 * n_wl;
+      const int cb = in.media_off + 5 * n_wl + (bsdf ? 4 : 0);
       std::vector<double> hdr(CO_HDR, 0.0);
       if (in.coating == OLB_COAT_THIN_FILM) {
         if (!in_pool(cb, 1)) { res.error = "thin-film block outside pool"; return res; }
@@ -683,6 +712,7 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
       features |= FEAT_POL | FEAT_JONES;
       res.bwd_supported = false;       // the adjoint has no polarization
     }
+    if (bsdf) pool.insert(pool.end(), bsdf_block, bsdf_block + BS_LEN);
     o.media_off = (int)pool.size();
     bool absorbing = false;
     for (int j = 0; j < n_wl; ++j) {
@@ -820,6 +850,10 @@ static BatchPrep prepare_batch(const OlbTable& tmpl, const double* params, int n
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].interaction != OLB_INTERACT_REFRACT) {
       out.error = "batched tables with phase-profile or grating surfaces are not built"; out.unsupported = true; return out;
+    }
+  for (int s = 0; s < S && tmpl.surfaces; ++s)
+    if (tmpl.surfaces[s].flags & OLB_SF_BSDF) {
+      out.error = "batched tables with BSDF surfaces are not built"; out.unsupported = true; return out;
     }
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].kind == OLB_GEOM_GRID_SAG) {

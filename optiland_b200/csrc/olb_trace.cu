@@ -23,6 +23,7 @@
 
 #include "../../include/olb.h"
 #include "olb_math.cuh"
+#include "olb_bsdf.cuh"
 #include "olb_prep.h"
 
 namespace olb {
@@ -91,6 +92,9 @@ struct TraceArgs {
   int32_t pol_mode; int32_t pol_pad;
   double pol_ax[2], pol_ay[2];     // complex amplitudes Ex e^{i phase_x}, Ey e^{i phase_y}
   void* pol_i;                     // optional separate output of the updated intensity
+  // BSDF scatter draws (FEAT_BSDF kernels): ray index = ray0 + index in this call's arrays, Philox counter word
+  int64_t ray0;
+  uint32_t rng_stream; int32_t rng_pad;
 };
 
 // Shared-memory slots per thread of a polarized kernel: the P matrix (18) + launch direction (3) + launch intensity
@@ -279,6 +283,10 @@ __global__ void __launch_bounds__(BLOCK, (MinBlocks<T, RPT, FEAT>::v)) trace_ker
       }
 #pragma unroll
       for (int k = 0; k < RPT; ++k) { r[k].opd_lo = 0; r[k].widx = 0; r[k].L0 = r[k].M0 = r[k].N0 = 0; }
+      if constexpr ((FEAT & FEAT_BSDF) != 0) {
+#pragma unroll
+        for (int k = 0; k < RPT; ++k) { r[k].id = (uint64_t)(a.ray0 + base + k); r[k].stream = a.rng_stream; }
+      }
       if (n_wl > 1) {
         load_rays<T, RPT>((const T*)a.w, bin, valid, v);
 #pragma unroll
@@ -864,6 +872,7 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       // lean polarized variants for the common systems: the general kernel's code does not fit the instruction
       // cache (no_instruction was the second largest stall of the Zernike + Fresnel configuration)
       const uint32_t g = features & ~FEAT_POL;
+      if (g & FEAT_BSDF) return fail(OLB_ERR_UNSUPPORTED, "polarized trace of a table with a BSDF surface is not built");
       if (g & FEAT_POLYGON)      // polygon apertures: the grid-sag superset + the polygon scan, so a polygon works on any surface
         return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES | FEAT_GRID | FEAT_POLYGON>(a, stream);
       if (g & FEAT_GRID)         // grid-sag surfaces: the superset below, so every coating and DOE works on a grid
@@ -883,7 +892,10 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
   }
   // phase-profile tables: the general kernel plus the phase interaction, one ray per thread for either caller RPT;
   // tables with a ruled grating (phase surfaces allowed beside it) add the grating interaction to that, and tables with
-  // a grid-sag surface the grid loop to both; tables with a polygon aperture the polygon scan to all three
+  // a grid-sag surface the grid loop to both; tables with a polygon aperture the polygon scan to all three; tables with
+  // a BSDF surface the scatter to all four, so a BSDF works on every geometry, interaction and aperture
+  if (features & FEAT_BSDF)
+    return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON | FEAT_BSDF>(a, stream);
   if (features & FEAT_POLYGON)
     return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON>(a, stream);
   if (features & FEAT_GRID) return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID>(a, stream);
@@ -907,7 +919,7 @@ static int launch_feat_cf(const TraceArgs& a, uint32_t features, cudaStream_t st
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 template <typename T>
-static int trace_impl(const OlbDeviceTable* wh, const OlbTraceCall& c, cudaStream_t stream) {
+static int trace_impl(const OlbDeviceTable* wh, const OlbTraceCall& c, cudaStream_t stream, int64_t ray0 = 0) {
   if (!wh || wh->magic != WS_MAGIC || !wh->workspace)
     return fail(OLB_ERR_INVALID_ARG, "table handle was not initialised by olb_table_upload");
   const unsigned char* workspace_dev = (const unsigned char*)wh->workspace;
@@ -953,6 +965,8 @@ static int trace_impl(const OlbDeviceTable* wh, const OlbTraceCall& c, cudaStrea
   a.L0 = rays->L0; a.M0 = rays->M0; a.N0 = rays->N0; a.p = rays->p;
   a.status = c.status;
   a.tflags = flags;
+  a.ray0 = ray0;
+  a.rng_stream = c.rng_stream;
   if (rays_per_system > 0) {
     if (wh->n_systems < 1 || n_rays != rays_per_system * (int64_t)wh->n_systems)
       return fail(OLB_ERR_INVALID_ARG, "batched trace: n_rays must equal rays_per_system * n_systems of the table");
@@ -1304,7 +1318,7 @@ static int trace_host_impl(const OlbDeviceTable* table, int32_t first, int32_t l
     OlbTraceCall call{};
     call.first = first; call.last = last; call.n_rays = m; call.flags = flags & ~uint32_t(OLB_TF_NO_FINAL);
     call.rays = &d; call.rec = rp; call.launch = launch ? &dl : nullptr; call.status = status;
-    result = trace_impl<T>(&wh, call, q);
+    result = trace_impl<T>(&wh, call, q, done);   // BSDF draws: stream 0, ray indices of the whole host array
     if (result) break;
     for (int k = 0; k < 9; ++k) {
       if (k == 7) continue;

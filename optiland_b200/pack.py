@@ -430,8 +430,46 @@ def pack_jones_coating(spec: T.SurfaceSpec, coating, wavelengths) -> None:
         spec.jones_axis = _jones_axis(jones)
 
 
-def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
-    """One Optiland ``Surface`` / ``ObjectSurface`` / ``ImageSurface`` -> ``SurfaceSpec``."""
+def _mix64(v: int) -> int:
+    """SplitMix64's finaliser: a bijection of 64-bit integers that scatters nearby inputs."""
+    v &= (1 << 64) - 1
+    v = ((v ^ (v >> 30)) * 0xBF58476D1CE4E5B9) & ((1 << 64) - 1)
+    v = ((v ^ (v >> 27)) * 0x94D049BB133111EB) & ((1 << 64) - 1)
+    return v ^ (v >> 31)
+
+
+def pack_bsdf(bsdf, position: int = 0):
+    """(kind, sigma, key) of a surface's ``bsdf`` (optiland/scatter.py), None without one.  Only the two exact classes
+    are accepted: a subclass may override the scattering function.  A 64-bit seed is taken from torch's default
+    generator the first time the object is packed and kept on it, so every later trace of the same optic uploads the
+    same table (the per-call draws differ through OlbTraceCall.rng_stream), and ``torch.manual_seed`` before the optic
+    is built makes its traces repeat.  The Philox key mixes that seed with the surface's ``position`` in the table: one
+    BSDF object set on several surfaces draws independently at each of them, as the reference's sequential generator
+    does."""
+    if bsdf is None:
+        return None
+    name = _cls(bsdf)
+    if name == "LambertianBSDF":
+        kind, sigma = T.BSDF_LAMBERTIAN, 0.0
+    elif name == "GaussianBSDF":
+        kind, sigma = T.BSDF_GAUSSIAN, _f(bsdf.sigma)
+        if not math.isfinite(sigma):
+            raise UnsupportedSurface(f"bsdf GaussianBSDF with sigma {sigma}")
+    else:
+        raise UnsupportedSurface(f"bsdf scatter of class {name}")
+    seed = bsdf.__dict__.get("_olb_seed")
+    if seed is None:
+        import torch
+
+        lo, hi = (int(v) for v in torch.randint(0, 1 << 32, (2,), dtype=torch.int64))
+        seed = lo | (hi << 32)
+        bsdf.__dict__["_olb_seed"] = seed
+    return kind, sigma, _mix64(seed + (int(position) + 1) * 0x9E3779B97F4A7C15)
+
+
+def pack_surface(surface, wavelengths, position: int = 0) -> T.SurfaceSpec:
+    """One Optiland ``Surface`` / ``ObjectSurface`` / ``ImageSurface`` -> ``SurfaceSpec``; ``position``: its index in the
+    table being packed (it keys a BSDF's draws)."""
     sname = _cls(surface)
     n_wl = len(wavelengths)
     if sname == "ObjectSurface":
@@ -456,8 +494,7 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
 
     if grating is None and iname not in ("RefractiveReflectiveModel", "PhaseInteractionModel"):
         raise UnsupportedSurface(f"interaction model {iname}")
-    if getattr(im, "bsdf", None) is not None:
-        raise UnsupportedSurface("bsdf scatter")
+    bsdf = pack_bsdf(getattr(im, "bsdf", None), position)
     phase = pack_phase_profile(im.phase_profile) if iname == "PhaseInteractionModel" else None
 
     t_eff, R_eff = _pose(g.cs)
@@ -465,6 +502,8 @@ def pack_surface(surface, wavelengths) -> T.SurfaceSpec:
         raise UnsupportedSurface("non-finite pose")
 
     spec = T.SurfaceSpec(kind=kind, t=t_eff, R=R_eff, reflective=bool(im.is_reflective))
+    if bsdf is not None:
+        spec.bsdf, spec.bsdf_sigma, spec.bsdf_seed = bsdf
     if phase is not None:
         spec.interaction, spec.phase_terms, spec.phase_efficiency = phase
     if grating is not None:
@@ -557,7 +596,7 @@ def pack_surface_group(surface_group, wavelengths) -> T.SurfaceTable:
     if len(surfaces) > T.MAX_SURFACES:
         raise UnsupportedSurface(f"more than {T.MAX_SURFACES} surfaces")
     with _Prefetch(surfaces, wavelengths):
-        specs = [pack_surface(s, wavelengths) for s in surfaces]
+        specs = [pack_surface(s, wavelengths, j) for j, s in enumerate(surfaces)]
         nv = sum(T.polygon_vertices(s.aperture) for s in specs if s.aperture is not None)
         if nv > T.MAX_POLYGON_VERTICES:
             raise UnsupportedSurface(f"polygon apertures with {nv} vertices in all: more than {T.MAX_POLYGON_VERTICES} "

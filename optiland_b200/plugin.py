@@ -875,6 +875,12 @@ def _try_trace(backend, surfaces, rays, table_builder) -> bool:
     if not polarized and any(s.coating in T.JONES_COATINGS for s in table.surfaces):
         # the reference's ray generator raises for these too (ray_generator.py:90-94); RealRays pass them unchanged
         return _decline("thin-film, polarizer or retarder coating with unpolarized rays")
+    if any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
+        if polarized:
+            return _decline("BSDF scatter with polarized rays")
+        if _wants_grad(backend, surfaces, rays):
+            # the reference's eager path then runs its numba scatter (which does not take torch tensors)
+            return _decline("gradients wanted: BSDF scatter")
     launch_dir = (rays.L, rays.M, rays.N)
     if _wants_grad(backend, surfaces, rays):
         # gradients wanted: the records must be autograd outputs of the live parameter tensors
@@ -982,6 +988,8 @@ def install(engine=None, alias: str | None = None) -> None:
                 return _fused_decline(f"unsupported: {e}")
             if not polarized and any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces):
                 return None          # the reference raises for this combination (ray_generator.py:90-94)
+            if polarized and any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
+                return _fused_decline("BSDF scatter with polarized rays")
             if table.surfaces[0].kind != T.GEOM_NOOP:
                 return _fused_decline("first surface is not an object surface")
             rec = engine.trace_pupil(table, Px, Py, pupil_affine(sc), polarization=state) if polarized else \
@@ -1103,6 +1111,8 @@ def install(engine=None, alias: str | None = None) -> None:
                 return _fused_decline(f"unsupported: {e}")
             if not polarized and any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces):
                 return None          # the reference raises (ray_generator.py:90-94)
+            if polarized and any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
+                return _fused_decline("BSDF scatter with polarized rays")
             if table.surfaces[0].kind != T.GEOM_NOOP:
                 return _fused_decline("first surface is not an object surface")
             # (trace_generic does NOT run update_intensity, real_ray_tracer.py:143-152: P matrices only)
@@ -1172,6 +1182,8 @@ def install(engine=None, alias: str | None = None) -> None:
                 return _fused_decline(f"wavefront unsupported: {e}")
             if not polarized and any(s.coating in T.POLARIZING_COATINGS for s in table.surfaces):
                 return None
+            if polarized and any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
+                return _fused_decline("BSDF scatter with polarized rays")
             # steps 1-2, the reference's own code on ONE ray (strategy.py:160-170)
             chief = optic.trace_generic(*field, Px=0.0, Py=0.0, wavelength=wavelength)
             strategy._chief_ray = chief

@@ -44,6 +44,7 @@ SF_ROTATED = 1 << 1
 SF_APERTURE = 1 << 2
 SF_ABSORBING = 1 << 3
 SF_NORECORD = 1 << 4
+SF_BSDF = 1 << 5
 
 COAT_NONE = 0
 COAT_SIMPLE = 1
@@ -89,6 +90,13 @@ TF_POLARIZED = 1 << 0
 ST_ZERNIKE_RANGE = 1 << 0
 ST_CHEBYSHEV_RANGE = 1 << 1
 ST_K_PARALLEL_X = 1 << 2
+ST_BSDF_ATTEMPTS = 1 << 3
+
+# BSDF scatter (include/olb.h OLB_SF_BSDF): LambertianBSDF / GaussianBSDF, and the kernel's bound on the draws of one ray
+BSDF_NONE = 0
+BSDF_LAMBERTIAN = 1
+BSDF_GAUSSIAN = 2
+BSDF_MAX_ATTEMPTS = 65536
 
 MAX_SURFACES = 64
 MAX_WAVELENGTHS = 16
@@ -169,6 +177,11 @@ class SurfaceSpec:
     grid_x: np.ndarray = field(default_factory=lambda: np.zeros(0))
     grid_y: np.ndarray = field(default_factory=lambda: np.zeros(0))
     grid_sag: np.ndarray = field(default_factory=lambda: np.zeros((0, 0)))
+    # BSDF scatter (BSDF_LAMBERTIAN / BSDF_GAUSSIAN, include/olb.h): sigma (Gaussian) and the 64-bit Philox key of the
+    # surface's draws
+    bsdf: int = BSDF_NONE
+    bsdf_sigma: float = 0.0
+    bsdf_seed: int = 0
 
     def __post_init__(self):
         self.t = np.asarray(self.t, dtype=np.float64).reshape(3)
@@ -234,7 +247,16 @@ class SurfaceSpec:
             f |= SF_ABSORBING
         if not self.record:
             f |= SF_NORECORD
+        if self.bsdf != BSDF_NONE:
+            f |= SF_BSDF
         return f
+
+    def bsdf_block(self) -> np.ndarray:
+        """The pool block {kind, sigma, seed_lo, seed_hi} of a BSDF surface (include/olb.h), empty without one."""
+        if self.bsdf == BSDF_NONE:
+            return np.zeros(0)
+        seed = int(self.bsdf_seed)
+        return np.array([float(self.bsdf), float(self.bsdf_sigma), float(seed & 0xFFFFFFFF), float(seed >> 32)])
 
 
 def _polygon_operands(prog: np.ndarray, i: int) -> int:
@@ -326,6 +348,15 @@ class SurfaceTable:
                     raise ValueError("retarder: non-finite retardance")
                 if s.kind == GEOM_NOOP:
                     raise ValueError("polarizer / retarder on an object surface")
+            if s.bsdf != BSDF_NONE:
+                if s.bsdf not in (BSDF_LAMBERTIAN, BSDF_GAUSSIAN):
+                    raise ValueError(f"unknown BSDF kind {s.bsdf}")
+                if not np.isfinite(s.bsdf_sigma):
+                    raise ValueError(f"BSDF sigma {s.bsdf_sigma} must be finite")
+                if not 0 <= int(s.bsdf_seed) < 1 << 64:
+                    raise ValueError("BSDF seed must be a 64-bit unsigned integer")
+                if s.kind == GEOM_NOOP:
+                    raise ValueError("BSDF on an object surface")
             if s.kind == GEOM_GRID_SAG:
                 nx, ny = len(s.grid_x), len(s.grid_y)
                 if nx < 2 or ny < 2 or s.grid_sag.shape != (ny, nx):
@@ -423,8 +454,9 @@ class SurfaceTable:
                 ints["aper_len"][j] = len(s.aperture)
             cn1 = s.coat_n1 if s.coat_n1 is not None else s.n1
             cn2 = s.coat_n2 if s.coat_n2 is not None else s.n2
-            # a thin-film / polarizer / retarder block follows the media block directly (pool[media_off + 5 n_wl])
-            ints["media_off"][j] = push(np.concatenate([s.n1, s.n2, s.k1, cn1, cn2, s.coating_block()]))
+            # a BSDF block, then a thin-film / polarizer / retarder block follow the media block directly
+            # (pool[media_off + 5 n_wl])
+            ints["media_off"][j] = push(np.concatenate([s.n1, s.n2, s.k1, cn1, cn2, s.bsdf_block(), s.coating_block()]))
             assert len(s.n1) == n_wl
             if s.interaction == INTERACT_GRATING:
                 # the phase block's framing: "efficiency" 1 (the diffractive model has none), 3 terms {m, d, alpha}
@@ -525,6 +557,11 @@ class SurfaceTable:
             media = pool[m0: m0 + 5 * n_wl].reshape(5, n_wl)
             coating = int(r["coating"])
             cb = m0 + 5 * n_wl
+            bsdf = {}
+            if flags & SF_BSDF:
+                bsdf = dict(bsdf=int(pool[cb]), bsdf_sigma=float(pool[cb + 1]),
+                            bsdf_seed=int(pool[cb + 2]) | (int(pool[cb + 3]) << 32))
+                cb += 4
             film = {}
             if coating == COAT_THIN_FILM:
                 L = int(pool[cb])
@@ -564,6 +601,7 @@ class SurfaceTable:
                     **phase,
                     **film,
                     **grid,
+                    **bsdf,
                 )
             )
         return cls(specs, wavelengths)

@@ -14,6 +14,7 @@ box without CUDA or without the built library raises.
 from __future__ import annotations
 
 import ctypes as C
+import threading
 
 import numpy as np
 import torch
@@ -142,6 +143,7 @@ class DeviceTable:
         self.ready = torch.cuda.Event()
         self.ready.record(torch.cuda.current_stream(self.device))
         self.has_zernike = any(s.kind in (T.GEOM_ZERNIKE, T.GEOM_CHEBYSHEV) for s in table.surfaces)
+        self.has_bsdf = any(s.bsdf != T.BSDF_NONE for s in table.surfaces)
 
     @property
     def features(self) -> int:
@@ -158,7 +160,33 @@ def _pointer(s):
 
 def _status_word(dtab: "DeviceTable", device, force: bool = False):
     """Device int32 the kernels OR their OLB_ST_* bits into -- only for tables / call shapes that can raise them."""
-    return torch.zeros(1, dtype=torch.int32, device=device) if (dtab.has_zernike or force) else None
+    return torch.zeros(1, dtype=torch.int32, device=device) if (dtab.has_zernike or _has_bsdf(dtab) or force) else None
+
+
+def _has_bsdf(dtab) -> bool:
+    """Does the prepared table hold BSDF surfaces?  (Batched tables never do, and have no such attribute.)"""
+    return getattr(dtab, "has_bsdf", False)
+
+
+_STREAM = {"state": None, "next": 0}
+_STREAM_LOCK = threading.Lock()
+
+
+def next_rng_stream() -> int:
+    """The Philox counter word of one trace of a table with BSDF surfaces (OlbTraceCall.rng_stream).  A counter: each
+    call takes the next value, so successive calls never repeat a stream (up to 2^32 calls).  Its start is drawn from
+    torch's default generator whenever that generator's state is not the one this function left behind (first use,
+    ``torch.manual_seed``, other draws in between), so ``torch.manual_seed`` makes a sequence of traces repeat bit for
+    bit."""
+    g = torch.default_generator
+    with _STREAM_LOCK:
+        st = g.get_state()
+        if _STREAM["state"] is None or not torch.equal(st, _STREAM["state"]):
+            _STREAM["next"] = int(torch.randint(0, 1 << 32, (1,), dtype=torch.int64).item())
+            _STREAM["state"] = g.get_state()
+        s = _STREAM["next"]
+        _STREAM["next"] = (s + 1) & 0xFFFFFFFF
+        return s
 
 
 def _raise_status(status) -> None:
@@ -180,6 +208,10 @@ def _raise_status(status) -> None:
     if st & T.ST_K_PARALLEL_X:
         # optiland/rays/polarized_rays.py:216-218
         raise ValueError("k-vector parallel to x-axis is not currently supported.")
+    if st & T.ST_BSDF_ATTEMPTS:
+        # the reference would loop for ever (optiland/scatter.py); the kernel bounds the loop
+        raise ValueError(f"BSDF scatter: a ray rejected {T.BSDF_MAX_ATTEMPTS} drawn directions (is the Gaussian sigma "
+                         "far above 1?); its direction is NaN")
 
 
 def _out_buffer(k: int, rows: int, n: int, dtype, device) -> torch.Tensor:
@@ -206,17 +238,21 @@ def _take_last_row(rays, recs):
 
 
 def _trace(dtab, device, dtype, first, last, n, flags, rays=None, rec=None, launch=None, center=(0.0, 0.0),
-           moments=None, rays_per_system=0, wavefront=None, pol=None, status=None, own_status=True):
+           moments=None, rays_per_system=0, wavefront=None, pol=None, status=None, own_status=True, rng_stream=None):
     """The one forward call of the library (olb_trace_call_f32 / _f64, include/olb.h: OlbTraceCall).  ``rays`` /
     ``rec`` / ``launch`` / ``pol``: ctypes structs or None; ``wavefront``: (OlbWavefrontRef, OlbWavefrontOut) or None;
     ``moments``: device tensor or None.  ``own_status``: the status word is made here (when the table or the call
     shape can set OLB_ST_* bits) and the reference's errors are raised from it; otherwise ``status`` (a caller-owned
-    device int32, or None) is passed through unchecked."""
+    device int32, or None) is passed through unchecked.  ``rng_stream``: the counter word of BSDF scatter draws (tables
+    with BSDF surfaces; None draws a fresh one, ``next_rng_stream``)."""
+    if _has_bsdf(dtab) and rng_stream is None:
+        rng_stream = next_rng_stream()
     if own_status:
         status = _status_word(dtab, device, force=pol is not None)
     ref, out = wavefront if wavefront is not None else (None, None)
     call = _lib.OlbTraceCall(
-        first=first, last=last, n_rays=n, flags=flags, rays=_pointer(rays), rec=_pointer(rec), launch=_pointer(launch),
+        first=first, last=last, n_rays=n, flags=flags, rng_stream=int(rng_stream or 0), rays=_pointer(rays),
+        rec=_pointer(rec), launch=_pointer(launch),
         center=(float(center[0]), float(center[1])), moments=moments.data_ptr() if moments is not None else None,
         rays_per_system=rays_per_system, wavefront_ref=_pointer(ref), wavefront_out=_pointer(out), pol=_pointer(pol),
         status=status.data_ptr() if status is not None else None)
@@ -244,7 +280,7 @@ def _c_polarization(state, intensity_out=None):
 
 
 def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, record: bool = True,
-                 want_l0: bool = False, polarization=False):
+                 want_l0: bool = False, polarization=False, rng_stream=None):
     """One trace of ``rays`` on the device.  Returns the dict of (rows, N) record tensors (or None).
 
     With ``record`` the final state is NOT written a second time: ``rays.x`` .. ``rays.opd``
@@ -255,6 +291,8 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
     ``polarization`` (PolarizedRays only): None / "unpolarized" / (Ex, Ey, phase_x, phase_y) runs
     PolarizedRays.update_intensity as the kernel's epilogue (OlbTraceCall.pol): ``rays.i`` becomes
     sum |P E0|^2 i0 / n_states while the record rows keep the geometric intensity.
+
+    ``rng_stream``: BSDF tables only, the counter word of the scatter draws (None: ``next_rng_stream()``).
     """
     n = len(rays)
     if rays.device != dtab.device:
@@ -293,7 +331,7 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
             raise ValueError("the intensity epilogue needs PolarizedRays")
         pol_i = torch.empty_like(rays.x)
         c_pol = _c_polarization(polarization, pol_i)
-    _trace(dtab, rays.device, rays.dtype, first, last, n, flags, rays=c_rays, rec=c_rec, pol=c_pol)
+    _trace(dtab, rays.device, rays.dtype, first, last, n, flags, rays=c_rays, rec=c_rec, pol=c_pol, rng_stream=rng_stream)
     if recs is not None:
         _take_last_row(rays, recs)
     if pol_i is not None:
@@ -547,9 +585,13 @@ def trace_host(dtab: DeviceTable, h_in: dict, h_out: dict, n: int, dtype=torch.f
         c_in = _lib.OlbRays(**{k: h_in[k].data_ptr() for k in ("x", "y", "z", "L", "M", "N", "i")},
                             w=h_in["w"].data_ptr() if "w" in h_in and dtab.table.n_wl > 1 else None)
     c_rec = _c_records(rec) if rec is not None else None
+    # BSDF tables: the attempt bound's status bit (the other OLB_ST_* bits are not collected on this path)
+    status = torch.zeros(1, dtype=torch.int32, device=dtab.device) if _has_bsdf(dtab) else None
     with torch.cuda.device(dtab.device):
         rc = getattr(lib, f"olb_trace_host_{sfx}")(
             C.byref(dtab.c), first, last, _byref(la), _byref(c_in), C.byref(c_out), _byref(c_rec), n, chunk,
-            C.c_void_p(scratch.data_ptr()), scratch.numel(), 0, None)
+            C.c_void_p(scratch.data_ptr()), scratch.numel(), 0,
+            C.c_void_p(status.data_ptr()) if status is not None else None)
     _lib.check(rc, f"olb_trace_host_{sfx}")
+    _raise_status(status)
     return scratch
