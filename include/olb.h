@@ -412,6 +412,10 @@ typedef struct OlbRecords {
                                           reference raises ValueError (optiland/rays/polarized_rays.py:216-218)     */
 #define OLB_ST_BSDF_ATTEMPTS (1 << 3)   /* a BSDF scatter drew OLB_BSDF_MAX_ATTEMPTS rejected directions; that ray's
                                           direction is NaN (the reference would loop for ever, scatter.py)        */
+#define OLB_ST_AIM_NAN_START (1 << 4)   /* olb_aim_*: some ray's initial x error is NaN; the reference raises ValueError
+                                          (optiland/rays/ray_aiming/iterative.py:141-145)                          */
+#define OLB_ST_AIM_UNCONVERGED (1 << 5) /* olb_aim_*: some ray is not converged after max_iter steps; the reference
+                                          raises ValueError (iterative.py:278-279)                                 */
 
 int olb_version(void);
 /* Copies the calling thread's last error message into buf (NUL terminated). */
@@ -729,6 +733,44 @@ typedef struct OlbTraceCall {
 } OlbTraceCall;               /* 112 bytes                                                                      */
 int olb_trace_call_f32(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream);
 int olb_trace_call_f64(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream);
+
+/*
+ * Ray-aiming solve: one call of Optiland's IterativeRayAimer.aim_rays from a given guess
+ * (optiland/rays/ray_aiming/iterative.py:60-281), each ray solved by its own thread with no host round trip.  A ray's
+ * iterates do not depend on the other rays': a converged ray keeps its parameters, a non-converged ray takes its own
+ * step, a NaN ray never converges.  For each ray, in the element type and in the reference's operation order:
+ *   trace       the launch state (intensity 1, OPD 0) through surfaces [first, last) of the prepared table (first = 1
+ *               for an infinite object, else 0; last = stop + 1; surface last - 1 must not be the object surface) and
+ *               take its intercept (x_s, y_s) in the local frame of surface last - 1;
+ *   error       e = (x_s - Px r_stop, y_s - Py r_stop); converged when ex^2 + ey^2 < tol^2;
+ *   Jacobian    J = diag(J_factor) at the start;
+ *   step        det = J11 J22 - J12 J21 (1e-12 when |det| < 1e-12),
+ *               dp1 = -(J22 ex + (-J12) ey) / det,  dp2 = -((-J21) ex + J11 ey) / det;
+ *               infinite: (x, y) += dp;  finite: (L, M) += dp, N unchanged and not renormalised (as the reference);
+ *   update      after the re-trace, J += (dE - J dp) dp^T / max(|dp|^2, 1e-20) (Broyden, with the old J);
+ * at most max_iter steps.  The solution is written in place into the guess arrays (x, y or L, M).
+ * Status bits OR-ed into `status`: OLB_ST_AIM_NAN_START, OLB_ST_AIM_UNCONVERGED, and the trace's own
+ * OLB_ST_ZERNIKE_RANGE / OLB_ST_CHEBYSHEV_RANGE; each is a ValueError of the reference, i.e. a failed solve.
+ * Tables with a BSDF surface, or needing polarized rays, are OLB_ERR_UNSUPPORTED.  Launches one kernel (no records).
+ * Asynchronous on `stream`.
+ */
+typedef struct OlbAimCall {
+  int32_t first, last;
+  int64_t n_rays;
+  /* Device SoA, n_rays each: the guess x, y, z, L, M, N in global coordinates (updated in place), plus w when the
+   * table has several wavelengths.  i, opd, L0..N0 and p are not read.  16-byte aligned. */
+  const OlbRays* rays;
+  const void* Px;             /* device, n_rays normalised pupil targets of the element type; 16-byte aligned      */
+  const void* Py;
+  double r_stop;              /* stop radius of the stop-size strategy                                            */
+  double J_factor;            /* initial Jacobian diagonal, the paraxial factor (|.| >= 1e-12 already applied)     */
+  double tol;                 /* convergence tolerance on the stop (tol^2 is formed in fp64)                      */
+  int32_t max_iter;
+  int32_t infinite;           /* 1: the object is at infinity, dp moves (x, y); 0: dp moves (L, M)                 */
+  int32_t* status;            /* device int32, OR-ed with OLB_ST_* bits (required)                                */
+} OlbAimCall;                 /* 80 bytes                                                                         */
+int olb_aim_f32(const OlbDeviceTable* table, const OlbAimCall* call, void* stream);
+int olb_aim_f64(const OlbDeviceTable* table, const OlbAimCall* call, void* stream);
 
 /*
  * Huygens-Fresnel PSF summation (SURVEY.md 8f-3; reference: NumbaSummation._huygens_fresnel_summation,

@@ -85,6 +85,12 @@ class OlbTraceCall(C.Structure):
                 ("status", C.c_void_p)]
 
 
+class OlbAimCall(C.Structure):
+    _fields_ = [("first", C.c_int32), ("last", C.c_int32), ("n_rays", C.c_int64), ("rays", C.POINTER(OlbRays)),
+                ("Px", C.c_void_p), ("Py", C.c_void_p), ("r_stop", C.c_double), ("J_factor", C.c_double),
+                ("tol", C.c_double), ("max_iter", C.c_int32), ("infinite", C.c_int32), ("status", C.c_void_p)]
+
+
 class OlbIrradiance(C.Structure):
     _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("z", C.c_void_p), ("i", C.c_void_p), ("n_rays", C.c_int64),
                 ("frame", C.c_int32), ("nx", C.c_int32), ("ny", C.c_int32), ("path", C.c_int32),
@@ -116,6 +122,8 @@ SYMBOLS = {
     "olb_table_upload": (C.c_int, [_P(OlbTable), C.c_void_p, C.c_int64, C.c_void_p, _P(OlbDeviceTable)]),
     "olb_trace_call_f32": (C.c_int, [_P(OlbDeviceTable), _P(OlbTraceCall), C.c_void_p]),
     "olb_trace_call_f64": (C.c_int, [_P(OlbDeviceTable), _P(OlbTraceCall), C.c_void_p]),
+    "olb_aim_f32": (C.c_int, [_P(OlbDeviceTable), _P(OlbAimCall), C.c_void_p]),
+    "olb_aim_f64": (C.c_int, [_P(OlbDeviceTable), _P(OlbAimCall), C.c_void_p]),
     "olb_trace_bwd_f32": (C.c_int, [_P(OlbDeviceTable), C.c_int32, C.c_int32, _P(OlbRays), _P(OlbRecords),
                                     _P(OlbRecords), _P(OlbRays), C.c_void_p, C.c_void_p, C.c_int64, C.c_uint64,
                                     C.c_void_p]),

@@ -24,6 +24,7 @@
 #include "../../include/olb.h"
 #include "olb_math.cuh"
 #include "olb_bsdf.cuh"
+#include "olb_aim.cuh"
 #include "olb_prep.h"
 
 namespace olb {
@@ -1087,6 +1088,111 @@ static int trace_impl(const OlbDeviceTable* wh, const OlbTraceCall& c, cudaStrea
   return launch_feat<T, 1>(a, features, stream);
 }
 
+// ---- ray-aiming solve (OlbAimCall, olb_aim.cuh) ----------------------------------------------
+struct AimArgs {
+  const unsigned char* blob;
+  int32_t blob_bytes;
+  int32_t first, last;
+  int32_t max_iter, infinite;
+  int64_t n_rays;
+  void* x; void* y; void* z; void* L; void* M; void* N; const void* w;
+  const void* px; const void* py;
+  double r_stop, J_factor, tol_sq;
+  int32_t* status;
+};
+
+// One ray per thread, grid-stride; the table is staged in shared memory as in trace_kernel.  Writes only the two
+// solved parameters of each ray and the status word.
+template <typename T, uint32_t FEAT>
+__global__ void __launch_bounds__(BLOCK) aim_kernel(const __grid_constant__ AimArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem);
+  unsigned char* tab = smem + 16;
+  stage_table(tab, a.blob, (uint32_t)a.blob_bytes, bar);
+  const PrepHeader* H = reinterpret_cast<const PrepHeader*>(tab);
+  const PrepSurface<T>* surf = reinterpret_cast<const PrepSurface<T>*>(tab + sizeof(PrepHeader));
+  const T* pool = reinterpret_cast<const T*>(surf + H->n_surf);
+  const T* wl = pool + H->pad[0];
+  const T r_stop = (T)a.r_stop, Jf = (T)a.J_factor, tol_sq = (T)a.tol_sq;
+  const bool inf = a.infinite != 0;
+  int status = 0;
+  for (int64_t k = (int64_t)blockIdx.x * BLOCK + threadIdx.x; k < a.n_rays; k += (int64_t)gridDim.x * BLOCK) {
+    T x = ((const T*)a.x)[k], y = ((const T*)a.y)[k], z = ((const T*)a.z)[k];
+    T L = ((const T*)a.L)[k], M = ((const T*)a.M)[k], N = ((const T*)a.N)[k];
+    const int widx = H->n_wl > 1 ? aim_widx<T>(wl, H->n_wl, ((const T*)a.w)[k]) : 0;
+    const T tx = o_mul_nc(((const T*)a.px)[k], r_stop), ty = o_mul_nc(((const T*)a.py)[k], r_stop);
+    status |= aim_ray<T, FEAT>(surf, pool, a.first, a.last, x, y, z, L, M, N, widx, tx, ty, Jf, tol_sq, a.max_iter, inf);
+    if (inf) { ((T*)a.x)[k] = x; ((T*)a.y)[k] = y; }
+    else { ((T*)a.L)[k] = L; ((T*)a.M)[k] = M; }
+  }
+  if (status != 0) atomicOr(a.status, status);
+}
+
+template <typename T, uint32_t FEAT>
+static int launch_aim(const AimArgs& a, cudaStream_t stream) {
+  auto kern = aim_kernel<T, FEAT>;
+  const size_t smem = 16 + (size_t)a.blob_bytes;
+  static thread_local int cached_dev = -1;
+  static thread_local int num_sms = 0;
+  static thread_local int blocks_per_sm = 0;
+  static thread_local size_t cached_smem = 0;
+  int dev = 0;
+  OLB_CUDA(cudaGetDevice(&dev));
+  if (dev != cached_dev || smem != cached_smem) {
+    if (smem > 48 * 1024) OLB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    OLB_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+    OLB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, BLOCK, smem));
+    if (blocks_per_sm < 1) return fail(OLB_ERR_CUDA, "aim kernel does not fit on an SM (table too large?)");
+    cached_dev = dev;
+    cached_smem = smem;
+  }
+  // one resident wave at most: each CTA stages the table once and then strides over the rays
+  int64_t grid = (a.n_rays + BLOCK - 1) / BLOCK;
+  const int64_t wave = (int64_t)num_sms * blocks_per_sm;
+  if (grid > wave) grid = wave;
+  kern<<<(unsigned)grid, BLOCK, smem, stream>>>(a);
+  OLB_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return OLB_OK;
+}
+
+template <typename T>
+static int aim_impl(const OlbDeviceTable* wh, const OlbAimCall& c, cudaStream_t stream) {
+  if (!wh || wh->magic != WS_MAGIC || !wh->workspace)
+    return fail(OLB_ERR_INVALID_ARG, "table handle was not initialised by olb_table_upload");
+  if (wh->n_systems > 1) return fail(OLB_ERR_UNSUPPORTED, "ray aiming on a batched table is not built");
+  if (c.n_rays < 0) return fail(OLB_ERR_INVALID_ARG, "n_rays < 0");
+  if (c.first < 0 || c.last > wh->n_surfaces || c.first >= c.last) return fail(OLB_ERR_INVALID_ARG, "bad surface range");
+  if (c.max_iter < 0) return fail(OLB_ERR_INVALID_ARG, "max_iter < 0");
+  if (!c.status) return fail(OLB_ERR_INVALID_ARG, "status is NULL");
+  const int variant = aim_variant(wh->features);
+  if (variant < 0) return fail(OLB_ERR_UNSUPPORTED, "ray aiming through a BSDF surface or a polarizing coating is not built");
+  if (c.n_rays == 0) return OLB_OK;
+  if (!c.rays) return fail(OLB_ERR_INVALID_ARG, "rays is NULL");
+  const OlbRays& r = *c.rays;
+  const void* req[] = {r.x, r.y, r.z, r.L, r.M, r.N, c.Px, c.Py};
+  for (const void* p : req) {
+    if (!p) return fail(OLB_ERR_INVALID_ARG, "a guess or pupil array is NULL");
+    if (!aligned16(p)) return fail(OLB_ERR_ALIGNMENT, "guess or pupil array not 16-byte aligned");
+  }
+  if (wh->n_wl > 1) {
+    if (!r.w) return fail(OLB_ERR_INVALID_ARG, "rays.w is NULL but the table has several wavelengths");
+    if (!aligned16(r.w)) return fail(OLB_ERR_ALIGNMENT, "rays.w not 16-byte aligned");
+  }
+  AimArgs a{};
+  a.blob = (const unsigned char*)wh->workspace + (sizeof(T) == 8 ? wh->off_f64 : wh->off_f32);
+  a.blob_bytes = sizeof(T) == 8 ? wh->bytes_f64 : wh->bytes_f32;
+  a.first = c.first; a.last = c.last; a.max_iter = c.max_iter; a.infinite = c.infinite ? 1 : 0;
+  a.n_rays = c.n_rays;
+  a.x = r.x; a.y = r.y; a.z = r.z; a.L = r.L; a.M = r.M; a.N = r.N; a.w = r.w;
+  a.px = c.Px; a.py = c.Py;
+  a.r_stop = c.r_stop; a.J_factor = c.J_factor; a.tol_sq = c.tol * c.tol;
+  a.status = c.status;
+  if (variant == AIM_CLOSED_FORM) return launch_aim<T, FEAT_ROT>(a, stream);
+  if (variant == AIM_GENERAL) return launch_aim<T, AIM_FEAT_GENERAL>(a, stream);
+  return launch_aim<T, AIM_FEAT_SUPERSET>(a, stream);
+}
+
 }  // namespace olb
 
 // =============================================================================================
@@ -1205,6 +1311,15 @@ int olb_trace_call_f32(const OlbDeviceTable* table, const OlbTraceCall* call, vo
 int olb_trace_call_f64(const OlbDeviceTable* table, const OlbTraceCall* call, void* stream) {
   if (!call) return fail(OLB_ERR_INVALID_ARG, "call is NULL");
   return trace_impl<double>(table, *call, (cudaStream_t)stream);
+}
+
+int olb_aim_f32(const OlbDeviceTable* table, const OlbAimCall* call, void* stream) {
+  if (!call) return fail(OLB_ERR_INVALID_ARG, "call is NULL");
+  return aim_impl<float>(table, *call, (cudaStream_t)stream);
+}
+int olb_aim_f64(const OlbDeviceTable* table, const OlbAimCall* call, void* stream) {
+  if (!call) return fail(OLB_ERR_INVALID_ARG, "call is NULL");
+  return aim_impl<double>(table, *call, (cudaStream_t)stream);
 }
 
 int olb_trace_bwd_f32(const OlbDeviceTable* table, int32_t first, int32_t last, const OlbRays* rays_in,

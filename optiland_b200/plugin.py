@@ -225,6 +225,18 @@ class CudaEngine:
         return rec
 
 
+    def aim(self, table: T.SurfaceTable, guess: dict, Px, Py, r_stop: float, J_factor: float, tol: float,
+            max_iter: int, infinite: bool) -> int:
+        """One ray-aiming solve through the whole ``table`` (olb_aim_*, one launch): ``guess`` holds the launch state
+        {"x" .. "N"} (+ "w" for several wavelengths) as aligned device tensors and receives the solution in place.
+        Returns the OLB_ST_* bits (one 4-byte read-back); any bit set is a failed solve."""
+        from .trace import aim_device
+
+        dt = self.device_table(table, guess["x"].device)
+        self._note("aim", table.num_surfaces, int(guess["x"].numel()))
+        st = aim_device(dt, guess, Px, Py, 0, table.num_surfaces, r_stop, J_factor, tol, max_iter, infinite)
+        return int(st.item())
+
     def accepts_tensor(self, t) -> bool:
         import torch
 
@@ -847,34 +859,47 @@ def _trace_grad_per_wavelength(engine, surfaces, rays, table_builder, wl):
     return rec
 
 
-def _try_trace(backend, surfaces, rays, table_builder) -> bool:
-    """Common body of the two wrappers.  ``surfaces``: the Surface objects to be traced (in
-    order); ``table_builder(wavelengths)`` packs them.  Returns False to decline."""
+def _trace_check(rays, table_builder):
+    """What every trace of ``rays`` through the capability needs: returns ``(table, wavelengths)``, or the reason (a
+    str) to decline.  ``table_builder(wavelengths)`` packs the surfaces.  Shared by ``_try_trace`` and the device ray
+    aimer, which launches on the table a subset trace would use."""
     polarized = type(rays).__name__ == "PolarizedRays"
     if type(rays).__name__ != "RealRays" and not polarized:
-        return _decline(f"ray class {type(rays).__name__}")  # ParaxialRays etc.: reference path
+        return f"ray class {type(rays).__name__}"  # ParaxialRays etc.: reference path
     engine = _state["engine"]
     if not engine.accepts(rays):
-        return _decline("rays not resident on a CUDA device (or not fp32/fp64)")
+        return "rays not resident on a CUDA device (or not fp32/fp64)"
     if not getattr(rays, "is_normalized", True):
         # a previous surface left un-normalised direction cosines (thin_lens_interaction_model.py:111) and
         # HomogeneousPropagation.propagate would renormalise them first (propagation/homogeneous.py:55-56); the
         # kernel assumes unit directions
-        return _decline("rays.is_normalized is False")
+        return "rays.is_normalized is False"
     wl = _unique_wavelengths(rays.w)
     if wl is None:
-        return _decline(f"more than {T.MAX_WAVELENGTHS} distinct wavelengths")
+        return f"more than {T.MAX_WAVELENGTHS} distinct wavelengths"
     try:
         table = table_builder(wl)
         _prepare(engine, table, rays.x.device)         # upload errors (OlbError) decline as well
     except _PACK_ERRORS as e:
-        return _decline(f"unsupported: {e}")
+        return f"unsupported: {e}"
     if not polarized and any(s.coating == T.COAT_FRESNEL for s in table.surfaces):
         # the reference raises for this combination (ray_generator.py:90-94)
-        return _decline("Fresnel coating with unpolarized rays")
+        return "Fresnel coating with unpolarized rays"
     if not polarized and any(s.coating in T.JONES_COATINGS for s in table.surfaces):
         # the reference's ray generator raises for these too (ray_generator.py:90-94); RealRays pass them unchanged
-        return _decline("thin-film, polarizer or retarder coating with unpolarized rays")
+        return "thin-film, polarizer or retarder coating with unpolarized rays"
+    return table, wl
+
+
+def _try_trace(backend, surfaces, rays, table_builder) -> bool:
+    """Common body of the two wrappers.  ``surfaces``: the Surface objects to be traced (in
+    order); ``table_builder(wavelengths)`` packs them.  Returns False to decline."""
+    polarized = type(rays).__name__ == "PolarizedRays"
+    checked = _trace_check(rays, table_builder)
+    if isinstance(checked, str):
+        return _decline(checked)
+    table, wl = checked
+    engine = _state["engine"]
     if any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
         if polarized:
             return _decline("BSDF scatter with polarized rays")
@@ -914,6 +939,174 @@ def _try_trace(backend, surfaces, rays, table_builder) -> bool:
     return True
 
 
+def _capture_warnings(caught) -> list:
+    """``warnings.catch_warnings(record=True)`` records as (message, category, filename, lineno, module name, registry):
+    enough to issue each again as the original ``warnings.warn`` call issued it, through the same filters and the
+    once-per-location registry of the module it was attributed to."""
+    by_file = {getattr(m, "__file__", None): m for m in list(sys.modules.values())}
+    out = []
+    for w in caught:
+        mod = by_file.get(w.filename)
+        reg = mod.__dict__.setdefault("__warningregistry__", {}) if mod is not None else None
+        out.append((w.message, w.category, w.filename, w.lineno, getattr(mod, "__name__", None), reg))
+    return out
+
+
+class _DeviceAimSolver:
+    """The solves of ONE ``RobustRayAimer.aim_rays`` call on the device.  Each is what ``IterativeRayAimer.aim_rays(...,
+    initial_guess=guess)`` computes (rays/ray_aiming/iterative.py:60-281) as ONE ``engine.aim`` launch plus one status
+    read.  The stop radius and the paraxial Jacobian factor depend on the optic alone, which does not change during the
+    call (the premise of _FrozenTables), so they are computed once; warnings the stop-radius strategy issued are issued
+    again on every solve, as the reference recomputes the radius per solve."""
+
+    def __init__(self, engine, table, r_stop, J_factor, tol, max_iter, infinite, warned):
+        self.engine, self.table = engine, table
+        self.r_stop, self.J_factor, self.tol, self.max_iter, self.infinite = r_stop, J_factor, tol, max_iter, infinite
+        self.warned = warned
+        self.wavelengths = None
+
+    def solve(self, pupil, guess):
+        """The solution (x, y, z, L, M, N) for the pupil targets ``pupil`` from ``guess``, or None where the reference
+        raises ValueError (NaN start, not converged, a freeform range error)."""
+        import warnings
+
+        import torch
+
+        import optiland.backend as be
+
+        for message, category, filename, lineno, module, registry in self.warned:
+            warnings.warn_explicit(message, category, filename, lineno, module=module, registry=registry)
+        ts = torch.broadcast_tensors(*[be.as_array_1d(v).detach() for v in guess])
+        dt, n = ts[0].dtype, ts[0].numel()
+
+        def fresh(t):               # a new, contiguous (hence 16-byte aligned) array: the caller's guess is not written
+            return t.detach().to(dt).expand(n).clone(memory_format=torch.contiguous_format)
+
+        sol = {k: fresh(t) for k, t in zip(("x", "y", "z", "L", "M", "N"), ts)}
+        if self.table.n_wl > 1:
+            sol["w"] = fresh(be.as_array_1d(self.wavelengths))
+        Px, Py = (fresh(be.as_array_1d(p)) for p in pupil)
+        status = self.engine.aim(self.table, sol, Px, Py, self.r_stop, self.J_factor, self.tol, self.max_iter,
+                                 self.infinite)
+        if status:
+            return None
+        return sol["x"], sol["y"], sol["z"], sol["L"], sol["M"], sol["N"]
+
+
+def _device_aim_solver(backend, aimer, probe, wavelengths):
+    """The ``_DeviceAimSolver`` of one ``RobustRayAimer.aim_rays`` call, or None to run the reference's body: an engine
+    without ``aim``, gradients wanted (the eager Broyden loop over the adjoint), or a subset table the capability declines
+    (the same checks as every trace, ``_trace_check``, on the table ``aimer_trace_subset`` would launch).  ``probe``: a
+    launch state of the call's rays (the first guess)."""
+    import warnings
+
+    import optiland.backend as be
+    from optiland.rays import RealRays
+    from optiland.rays.ray_aiming.initialization import get_stop_radius_strategy
+
+    engine = _state["engine"]
+    if not hasattr(engine, "aim"):
+        return None
+    optic = aimer.optic
+    group = optic.surfaces
+    stop = group.stop_index
+    infinite = bool(getattr(optic.object_surface, "is_infinite", False))
+    start = 1 if infinite else 0
+    surfaces = list(group.surfaces)[start:stop + 1]
+    if not surfaces:
+        return None
+    x, y, z, L, M, N = (be.as_array_1d(v) for v in probe)
+    rays = RealRays(x, y, z, L, M, N, intensity=be.ones_like(x), wavelength=wavelengths)
+    if _wants_grad(backend, surfaces, rays):
+        _decline("robust ray aiming: gradients wanted")
+        return None
+    checked = _trace_check(rays, _group_table_builder(group, start, stop + 1))
+    if isinstance(checked, str):
+        return None                     # the reference's body runs; its subset traces decline with this reason
+    table = checked[0]
+    if any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
+        _decline("robust ray aiming: BSDF surface before the stop")
+        return None
+    if table.surfaces[-1].kind == T.GEOM_NOOP:
+        return None                     # the stop is the object surface: it has no local frame in the kernel
+    it = aimer._iterative
+    with warnings.catch_warnings(record=True) as caught:
+        warnings.simplefilter("always")
+        r_stop = float(get_stop_radius_strategy(optic, "iterative").calculate_stop_radius())
+    wl_mean = be.mean(wavelengths) if hasattr(wavelengths, "__len__") else wavelengths
+    J_factor = it._get_paraxial_jacobian(float(wl_mean), stop, infinite)
+    if abs(J_factor) < 1e-12:
+        J_factor = 1e-12
+    solver = _DeviceAimSolver(engine, table, r_stop, float(J_factor), it.tol, it.max_iter, infinite,
+                              _capture_warnings(caught))
+    solver.wavelengths = wavelengths
+    return solver
+
+
+def _robust_aim_device(backend, aimer, fields, wavelengths, pupil_coords, initial_guess):
+    """``RobustRayAimer.aim_rays`` (rays/ray_aiming/robust.py:61-171) with every solve on the device (one launch and one
+    status read each, ``_DeviceAimSolver``); the paraxial guesses, the predictor and the interval halving are the
+    reference's.  None: the reference's body runs instead (``_device_aim_solver``).
+
+    Side effect: afterwards the surfaces hold the records of the stop-radius strategy's one-ray trace, not those of the
+    last subset trace as after the reference's body.  Every caller in the reference traces again before it reads
+    records."""
+    def paraxial_at(t):                 # targets and paraxial solution at continuation parameter t
+        pt = (pupil_coords[0] * t, pupil_coords[1] * t)
+        ft = (fields[0] * t, fields[1] * t) if aimer.scale_fields else fields
+        return pt, aimer._paraxial.aim_rays(ft, wavelengths, pt)
+
+    anchor = paraxial_at(0.0)[1] if initial_guess is None else None
+    solver = _device_aim_solver(backend, aimer, initial_guess if initial_guess is not None else anchor, wavelengths)
+    if solver is None:
+        return None
+    if initial_guess is not None:
+        sol = solver.solve(pupil_coords, initial_guess)
+        if sol is not None:
+            return sol
+        anchor = paraxial_at(0.0)[1]
+    return _robust_interval(aimer, solver, paraxial_at, 0.0, 1.0, anchor, anchor)
+
+
+def _robust_interval(aimer, solver, paraxial_at, t0, t1, sol0, par0):
+    """``RobustRayAimer._solve``: the solution at t1 from the one at t0, halving [t0, t1] where a solve fails."""
+    import optiland.backend as be
+
+    if (t1 - t0) < 1e-3:
+        return sol0
+    pt, par1 = paraxial_at(t1)
+    # predictor: the paraxial solution at t1 plus the real - paraxial difference at t0
+    xg, yg, zg, Lg, Mg = (p1 + (s0 - p0) for p1, s0, p0 in zip(par1[:5], sol0[:5], par0[:5]))
+    sq = Lg**2 + Mg**2
+    if be.any(sq > 1.0):                # one decision for the whole batch, as in the reference
+        f = be.sqrt(sq)
+        Lg, Mg = Lg / f, Mg / f
+        sq = Lg**2 + Mg**2
+    Ng = be.sqrt(1.0 - sq)
+    Ng = be.where(par1[5] >= 0, Ng, -Ng)
+    if getattr(aimer.optic.object_surface, "is_infinite", False):
+        Lg, Mg, Ng = par1[3], par1[4], par1[5]   # the field angle fixes the direction
+    sol = solver.solve(pt, (xg, yg, zg, Lg, Mg, Ng))
+    if sol is not None:
+        return sol
+    tm = (t0 + t1) / 2.0
+    sol_m = _robust_interval(aimer, solver, paraxial_at, t0, tm, sol0, par0)
+    return _robust_interval(aimer, solver, paraxial_at, tm, t1, sol_m, paraxial_at(tm)[1])
+
+
+def _group_table_builder(surface_group, start: int, stop: int):
+    """``table_builder`` of surfaces [start, stop) of a SurfaceGroup: the whole group packed, then sliced (memoised
+    inside a _FrozenTables context)."""
+    def build(wl):
+        def pack():
+            full = pack_surface_group(surface_group, wl)
+            return T.SurfaceTable(full.surfaces[start:stop], full.wavelengths)
+
+        return _frozen(("group", id(surface_group), start, stop, tuple(float(w) for w in wl)), surface_group, pack)
+
+    return build
+
+
 def install(engine=None, alias: str | None = None) -> None:
     """Register the backend and wrap the two trace entry points (idempotent)."""
     import optiland.backend as be
@@ -934,15 +1127,7 @@ def install(engine=None, alias: str | None = None) -> None:
             surfaces = list(surface_group.surfaces)[start:stop]
             if not surfaces:
                 return False
-
-            def build(wl):
-                def pack():
-                    full = pack_surface_group(surface_group, wl)
-                    return T.SurfaceTable(full.surfaces[start:stop], full.wavelengths)
-
-                return _frozen(("group", id(surface_group), start, stop, tuple(float(w) for w in wl)), surface_group, pack)
-
-            return _try_trace(self, surfaces, rays, build)
+            return _try_trace(self, surfaces, rays, _group_table_builder(surface_group, start, stop))
 
         def trace_optic(self, tracer, Hx, Hy, wavelength, num_rays, distribution):
             """``RealRayTracer.trace`` for ONE field with the launch state generated on the device
@@ -1325,8 +1510,21 @@ def install(engine=None, alias: str | None = None) -> None:
                 return orig(self, *args, **kwargs)
         return aim_rays
 
-    for cls, orig in orig_aim.items():
-        cls.aim_rays = _make_aim(orig)
+    IterativeRayAimer.aim_rays = _make_aim(orig_aim[IterativeRayAimer])
+
+    # the robust aimer (ProjectionLens120FOV / 160FOV, WideAngle170FOV): every solve of its continuation is ONE launch of
+    # the aim kernel instead of an eager Newton-Broyden loop of subset traces (and a stop-radius trace per solve)
+    def robust_aim_rays(self, fields, wavelengths, pupil_coords, initial_guess=None):
+        with _FrozenTables():
+            backend = registry.get(be.get_backend())
+            if (hasattr(backend, "trace_surfaces") and _state.get("device_aim", True)
+                    and not getattr(_tls, "in_reference", False)):
+                sol = _robust_aim_device(backend, self, fields, wavelengths, pupil_coords, initial_guess)
+                if sol is not None:
+                    return sol
+            return orig_aim[RobustRayAimer](self, fields, wavelengths, pupil_coords, initial_guess)
+
+    RobustRayAimer.aim_rays = robust_aim_rays
 
     # f-3: the Huygens-Fresnel summation strategy of the torch backend (psf/huygens_fresnel_strategies.py:183-273)
     from optiland.psf.huygens_fresnel_strategies import TorchSummation
@@ -1433,7 +1631,7 @@ def install(engine=None, alias: str | None = None) -> None:
     RealRayTracer.trace_generic = tracer_generic
     _state.update(installed=True, orig_group_trace=orig_group_trace, orig_surface_trace=orig_surface_trace,
                   orig_tracer_trace=orig_tracer_trace, orig_tracer_generic=orig_tracer_generic, orig_hf_compute=orig_hf_compute, orig_chief_compute=orig_chief_compute,
-                  old_backend=old, alias=alias, fuse_launch=True, fuse_wavefront=True, fuse_spot=True, fuse_fft_psf=True, fuse_aimer=True, orig_trace_subset=orig_trace_subset, orig_aim=orig_aim, saved_spot=saved_spot, saved_fft=saved_fft,
+                  old_backend=old, alias=alias, fuse_launch=True, fuse_wavefront=True, fuse_spot=True, fuse_fft_psf=True, fuse_aimer=True, device_aim=True, orig_trace_subset=orig_trace_subset, orig_aim=orig_aim, saved_spot=saved_spot, saved_fft=saved_fft,
                   saved_irr=saved_irr,
                   orig_position=orig_position, fast_positions=True, memo_paraxial=True,
                   orig_paraxial=(orig_generate, orig_epl, orig_epd, orig_positions))

@@ -91,6 +91,8 @@ ST_ZERNIKE_RANGE = 1 << 0
 ST_CHEBYSHEV_RANGE = 1 << 1
 ST_K_PARALLEL_X = 1 << 2
 ST_BSDF_ATTEMPTS = 1 << 3
+ST_AIM_NAN_START = 1 << 4
+ST_AIM_UNCONVERGED = 1 << 5
 
 # BSDF scatter (include/olb.h OLB_SF_BSDF): LambertianBSDF / GaussianBSDF, and the kernel's bound on the draws of one ray
 BSDF_NONE = 0

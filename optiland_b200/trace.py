@@ -339,6 +339,32 @@ def trace_device(dtab: DeviceTable, rays: RealRays, first: int, last: int, recor
     return recs
 
 
+def aim_device(dtab: DeviceTable, guess: dict, Px: torch.Tensor, Py: torch.Tensor, first: int, last: int,
+               r_stop: float, J_factor: float, tol: float, max_iter: int, infinite: bool) -> torch.Tensor:
+    """One ray-aiming solve on the device (olb_aim_f32 / _f64, include/olb.h: OlbAimCall).  ``guess``: the launch state
+    {"x", "y", "z", "L", "M", "N"} (+ "w" when the table has several wavelengths), 1-D device tensors of one type and
+    length, 16-byte aligned; the solution is written into them in place.  ``Px`` / ``Py``: the pupil targets, same type
+    and length.  Returns the device int32 status word (OLB_ST_* bits; not checked here, nothing is synchronised)."""
+    x = guess["x"]
+    n = int(x.numel())
+    for t in [guess[k] for k in ("y", "z", "L", "M", "N")] + [Px, Py]:
+        if t.dtype != x.dtype or t.device != dtab.device or t.numel() != n:
+            raise ValueError("aim: guess and pupil arrays must share one dtype, length and the table's device")
+    status = torch.zeros(1, dtype=torch.int32, device=dtab.device)
+    w = guess.get("w") if dtab.table.n_wl > 1 else None
+    c_rays = _lib.OlbRays(x=x.data_ptr(), y=guess["y"].data_ptr(), z=guess["z"].data_ptr(), L=guess["L"].data_ptr(),
+                          M=guess["M"].data_ptr(), N=guess["N"].data_ptr(), w=w.data_ptr() if w is not None else None)
+    call = _lib.OlbAimCall(first=first, last=last, n_rays=n, rays=C.pointer(c_rays), Px=Px.data_ptr(), Py=Py.data_ptr(),
+                           r_stop=float(r_stop), J_factor=float(J_factor), tol=float(tol), max_iter=int(max_iter),
+                           infinite=1 if infinite else 0, status=status.data_ptr())
+    sfx = _DTYPES[x.dtype]
+    with torch.cuda.device(dtab.device):
+        stream = torch.cuda.current_stream(dtab.device).cuda_stream
+        rc = getattr(dtab.lib, f"olb_aim_{sfx}")(C.byref(dtab.c), C.byref(call), C.c_void_p(stream))
+    _lib.check(rc, f"olb_aim_{sfx}")
+    return status
+
+
 def _aligned(t):
     """Contiguous and 16-byte aligned (a slice of a larger tensor may start anywhere; the C ABI wants aligned arrays)."""
     if t is None:
