@@ -111,9 +111,10 @@ def _zernike_stop(be, norm_radius):
     return zernike_singlet("fringe", norm_radius=norm_radius)
 
 
-def _aim_inputs(lens, hx, hy, t, wl=None, max_iter=None):
+def _aim_inputs(lens, hx, hy, t, wl=None, max_iter=None, pupil=None):
     """Everything one solve needs: the reference's aimer, its targets and paraxial guess, and the host solve's table
-    and scalars (computed as the plugin computes them)."""
+    and scalars (computed as the plugin computes them).  ``hx`` / ``hy``: one field or one per ray; ``pupil``: (px, py)
+    per ray (default: the 4-ring hexapolar pupil)."""
     import optiland.backend as be
     from optiland.rays.ray_aiming.initialization import get_stop_radius_strategy
     from optiland.rays.ray_aiming.iterative import IterativeRayAimer
@@ -124,10 +125,10 @@ def _aim_inputs(lens, hx, hy, t, wl=None, max_iter=None):
     it = IterativeRayAimer(lens)
     if max_iter is not None:
         it.max_iter = max_iter
-    px, py = _hexapolar()
+    px, py = _hexapolar() if pupil is None else pupil
     n = px.size
     Px, Py = be.array(px * t), be.array(py * t)
-    H = (be.array(np.full(n, hx * t)), be.array(np.full(n, hy * t)))
+    H = tuple(be.array(np.broadcast_to(np.asarray(h, dtype=np.float64) * t, (n,)).copy()) for h in (hx, hy))
     if wl is None:
         wl = lens.primary_wavelength
     guess = it._paraxial_aimer.aim_rays(H, wl, (Px, Py))
@@ -144,15 +145,21 @@ def _aim_inputs(lens, hx, hy, t, wl=None, max_iter=None):
     return dict(it=it, H=H, Px=Px, Py=Py, wl=wl, guess=guess, table=table, r_stop=r_stop, J=J, inf=inf)
 
 
-def _host_solve(a, guess=None, dtype=np.float64):
+def _host_solve(a, guess=None, dtype=np.float64, max_iter=None, ray_status=None):
+    """The host solve; ``ray_status`` (optional int32 array) receives each ray's status bits, whose OR must be the
+    status word."""
     import optiland.backend as be
 
     from oracle.hostcheck_aim import run_aim
 
     g = {k: be.to_numpy(be.as_array_1d(v)) for k, v in zip(KEYS, guess if guess is not None else a["guess"])}
     g["w"] = np.broadcast_to(be.to_numpy(be.as_array_1d(a["wl"])), g["x"].shape)
-    return run_aim(a["table"], g, be.to_numpy(a["Px"]), be.to_numpy(a["Py"]), 0, a["table"].num_surfaces, a["r_stop"],
-                   a["J"], a["it"].tol, a["it"].max_iter, a["inf"], dtype=dtype)
+    rs = ray_status if ray_status is not None else np.full(g["x"].size, -1, dtype=np.int32)
+    out = run_aim(a["table"], g, be.to_numpy(a["Px"]), be.to_numpy(a["Py"]), 0, a["table"].num_surfaces, a["r_stop"],
+                  a["J"], a["it"].tol, a["it"].max_iter if max_iter is None else max_iter, a["inf"], dtype=dtype,
+                  ray_status=rs)
+    assert int(np.bitwise_or.reduce(rs)) == out[1], (out[1], np.unique(rs))
+    return out
 
 
 def _reference_solve(a, guess=None):
@@ -309,23 +316,27 @@ class _Spy:
         monkeypatch.setattr(IterativeRayAimer, "_trace_subset", sub2)
 
 
-def _numpy_records(name, fields):
+def _numpy_records(name, fields, num_rays=4, distribution="hexapolar"):
     import optiland.backend as be
 
     be.set_backend("numpy")
     ref = _sample(name)
     out = []
     for hx, hy in fields:
-        ref.trace(hx, hy, ref.primary_wavelength, 4, "hexapolar")
+        ref.trace(hx, hy, ref.primary_wavelength, num_rays, distribution)
         out.append({k: np.array(getattr(ref.surfaces, k)) for k in ("x", "y", "z", "L", "M", "N", "opd", "intensity")})
     be.set_backend("torch")
     return out
 
 
 def _check_records(be, lens, want, what):
+    _check_record_arrays({k: be.to_numpy(getattr(lens.surfaces, k)) for k in want}, want, what)
+
+
+def _check_record_arrays(got, want, what):
     scale = max(1.0, float(np.nanmax(np.abs(np.where(np.isfinite(want["z"]), want["z"], 0.0)))))
     for k, v in want.items():
-        g = be.to_numpy(getattr(lens.surfaces, k))
+        g = got[k]
         assert np.array_equal(np.isnan(g), np.isnan(v)), (what, k)
         m = np.isfinite(v)
         assert not m.any() or float(np.max(np.abs(g[m] - v[m]))) <= 1e-10 * scale, (what, k)
