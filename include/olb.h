@@ -74,6 +74,37 @@ extern "C" {
 #define OLB_GEOM_GRID_SAG     11   /* bilinear interpolation of a table of sag values
                                       optiland/geometries/grid_sag.py:60-140 (see "Grid sag" below) */
 #define OLB_MAX_GRID_ELEMENTS 8192 /* per table: sum over grid surfaces of nx + ny + nx * ny (e.g. 89 x 89) */
+#define OLB_GEOM_FORBES_Q2D   12   /* conic + Forbes Q-2D freeform departure (see "Forbes Q-2D" below)
+                                      optiland/geometries/forbes/geometry.py:445-672, qpoly.py:286-540 */
+#define OLB_Q2D_MAX_M         16   /* highest azimuthal order m of a Q-2D surface                          */
+#define OLB_Q2D_MAX_TERMS     16   /* longest coefficient list (radial orders n = 0 .. 15) of any m         */
+#define OLB_MAX_Q2D_ELEMENTS  4096 /* per table: prepared Q-2D elements, sum over surfaces of
+                                      4 + n0 + sum_m (4 + 3 max(na_m, nb_m) + na_m + nb_m)                   */
+
+/*
+ * Forbes Q-2D (ForbesQ2dGeometry).  Pool block at coef_off, with aux0 = n0 (length of the m = 0 list) and n_coef = M
+ * (the highest azimuthal order, 0 <= M <= OLB_Q2D_MAX_M):
+ *   cm0[n0], then {na_m, nb_m} for m = 1 .. M, then the lists a_1[na_1], b_1[nb_1], a_2[na_2], b_2[nb_2], ...
+ * -- the reference's own grouping (cm0_coeffs, ams_coeffs[m-1], bms_coeffs[m-1]); every list may be empty and holds
+ * at most OLB_Q2D_MAX_TERMS finite values.  OlbSurface.norm_radius (> 0) is the normalisation radius; radius, conic, tol
+ * and max_iter are the base conic's and the Newton solver's.  The upload changes each list to the basis its Clenshaw
+ * recurrence runs on (m = 0: the Q-bfs change of FORBES_QBFS; m > 0: change_basis_q2d_to_pnm) and tabulates the
+ * recurrence constants abc_q2d_clenshaw(n, m), so the kernel does no per-(n, m) set-up.  With u = rho / norm_radius:
+ *   sag    z = z_base(r^2) + (u > 1 ? 0 : phi(r^2) [u^2 (1 - u^2) S_0(u^2) + sum_m u^m (cos m theta S_a,m + sin m theta S_b,m)])
+ *          with rho = sqrt(r^2 + 1e-12) and theta = atan2(y, x);
+ *   slopes d/dx, d/dy of the same with rho = sqrt(r^2) (no 1e-12); the departure's slopes are 0 where u > 1 (the base
+ *          conic remains; no range error); for rho < 1e-12 the slopes are the VERTEX value (S_a,1(0), S_b,1(0)) /
+ *          norm_radius, which ignores every other term;
+ *   sums   S = alpha_0 / 2 of the Clenshaw recurrence, minus 2/5 alpha_3 for m = 1 when the list has more than 3 terms
+ *          (q2d_sum_from_alphas);
+ *   base   z_base, its derivative and the conic-correction factor phi with the reference's clamps (1e-12, negative
+ *          radicand -> 0); an infinite radius gives z_base = 0 and phi = 1;
+ *   normal (fx, fy, -1) / |.| as for the other Newton families.
+ * A table with a Q-2D surface has bwd_supported = 0 and olb_table_upload_batch rejects it (OLB_ERR_UNSUPPORTED).  Its
+ * traces run two kernel variants of their own (plain and polarized); a Q-2D surface in a table that also has a phase
+ * profile, a ruled grating, a grid sag, a polygon aperture, a BSDF or a thin-film / polarizer / retarder coating is
+ * OLB_ERR_UNSUPPORTED at trace time, and so is ray aiming (olb_aim_*) through a Q-2D table.
+ */
 
 /*
  * Grid sag (GridSagGeometry).  Pool block at coef_off: x[nx], y[ny], sag[ny][nx] (row j holds y_j: sag_grid[j, i]);
@@ -346,6 +377,8 @@ typedef struct OlbSurface {
  *   FORBES_QBFS  : n_coef doubles a_0 .. a_M (missing radial orders = 0); OlbSurface.norm_radius = rho_max.
  *                  The change of basis to the Clenshaw form (geometries/forbes/qpoly.py:56-115) happens in
  *                  olb_table_upload.
+ *   FORBES_Q2D   : cm0[aux0], {na_m, nb_m} x n_coef, then the cosine / sine lists per m (see "Forbes Q-2D" above);
+ *                  OlbSurface.norm_radius = the normalisation radius.
  *   ZERNIKE      : n_coef terms, each 4 doubles {n, m, c*N_nm (sag), c (derivative)}
  *                  -- the reference's derivative path omits the normalisation
  *                  constant N_nm (optiland/zernike/base.py:104-136 vs :42-68);

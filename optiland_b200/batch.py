@@ -36,6 +36,8 @@ def template_params(table: T.SurfaceTable) -> np.ndarray:
         raise ValueError("batched tables with grid-sag surfaces are not built")
     if any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
         raise ValueError("batched tables with BSDF surfaces are not built")
+    if any(s.kind == T.GEOM_FORBES_Q2D for s in table.surfaces):
+        raise ValueError("batched tables with Forbes Q-2D surfaces are not built")
     p = np.zeros((table.num_surfaces, _lib.BP_COUNT))
     for s, spec in enumerate(table.surfaces):
         p[s, _lib.BP_TX:_lib.BP_TX + 3] = spec.t

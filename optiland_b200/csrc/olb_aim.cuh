@@ -18,13 +18,13 @@ namespace olb {
 
 // Kernel variant of an aim table (the trace kernel's instantiations, unpolarized): closed form, general, or the
 // phase / grating / grid-sag / polygon superset.  -1: not built (BSDF scatter; Fresnel / Jones coatings need
-// polarized rays, which the aimer never traces).
+// polarized rays, which the aimer never traces; Forbes Q-2D surfaces, whose code only the trace kernels carry).
 enum { AIM_CLOSED_FORM = 0, AIM_GENERAL = 1, AIM_SUPERSET = 2 };
 constexpr uint32_t AIM_FEAT_GENERAL = FEAT_ROT | FEAT_NEWTON | FEAT_EXTRA | FEAT_FREEFORM;
 constexpr uint32_t AIM_FEAT_SUPERSET = AIM_FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON;
 
 inline int aim_variant(uint32_t features) {
-  if (features & (FEAT_BSDF | FEAT_POL | FEAT_JONES)) return -1;
+  if (features & (FEAT_BSDF | FEAT_POL | FEAT_JONES | FEAT_Q2D)) return -1;
   if (features & (FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON)) return AIM_SUPERSET;
   if ((features & ~uint32_t(FEAT_ROT)) == 0) return AIM_CLOSED_FORM;
   return AIM_GENERAL;

@@ -465,11 +465,121 @@ OLB_HD void forbes_slopes(T x, T y, const PrepSurface<T>& S, const T* pool, T& f
   fy = df * o_div(y, rho);
 }
 
+// Forbes Q-2D freeform (include/olb.h "Forbes Q-2D"; forbes/geometry.py:539-672, qpoly.py:403-540), on the block
+// olb_prep.h prepares (Q2_*).  One list of one m: the Clenshaw recurrence of clenshaw_q2d / clenshaw_q2d_der,
+//   alpha_n = d_n + (A_n + B_n x) alpha_{n+1} - C_{n+1} alpha_{n+2},   alpha'_n = B_n alpha_{n+1} + (A_n + B_n x) alpha'_{n+1} - C_{n+1} alpha'_{n+2}
+// (alpha above the top term = 0), and the sums S = alpha_0 / 2, S' = alpha'_0 / 2, each minus 2/5 of its alpha_3 for m = 1
+// with more than 3 terms (q2d_sum_from_alphas).
+template <typename T, bool SLOPES>
+OLB_HD void q2d_list_sum(const T* d, const T* abc, int nl, bool m1, T x, T& S, T& dS) {
+  T a1 = 0, a2 = 0, d1 = 0, d2 = 0, a0 = 0, d0 = 0, a3 = 0, d3 = 0;
+  for (int n = nl - 1; n >= 0; --n) {
+    const T k = o_fma(abc[3 * n + 1], x, abc[3 * n]);
+    a0 = o_fma(k, a1, o_fma(-abc[3 * n + 2], a2, d[n]));
+    if (SLOPES) d0 = o_fma(abc[3 * n + 1], a1, o_fma(k, d1, -abc[3 * n + 2] * d2));
+    if (n == 3) { a3 = a0; d3 = d0; }
+    a2 = a1; a1 = a0; d2 = d1; d1 = d0;
+  }
+  const T q = (m1 && nl > 3) ? (T)0.4 : (T)0;
+  S = o_fma(-q, a3, (T)0.5 * a0);
+  if (SLOPES) dS = o_fma(-q, d3, (T)0.5 * d0);
+}
+// All m > 0 at one point (_compute_m_gt0_components, qpoly.py:422-459), with (c1, s1) = (cos, sin) theta:
+//   P = sum_m u^m (cos m theta S_a + sin m theta S_b)
+//   DR = sum_m u^(m-1) (cos m theta (2 x S'_a + m S_a) + sin m theta (2 x S'_b + m S_b)),  x = u^2  (dP/du)
+//   DT = sum_m m u^m (cos m theta S_b - sin m theta S_a)                                         (dP/dtheta)
+// cos m theta, sin m theta by rotation from (c1, s1).
+template <typename T, bool SLOPES>
+OLB_HD void q2d_angular(const T* p, int M, T u, T x, T c1, T s1, T& P, T& DR, T& DT) {
+  T cm = 1, sm = 0, um1 = 1;
+  P = 0; DR = 0; DT = 0;
+  for (int m = 1; m <= M; ++m) {
+    const T cn = o_fma(cm, c1, -sm * s1);
+    sm = o_fma(sm, c1, cm * s1);
+    cm = cn;
+    const T um = um1 * u;
+    const int na = (int)p[Q2_NA], nb = (int)p[Q2_NB], N = (int)p[Q2_N];
+    const T* abc = p + Q2_MHDR;
+    const T* da = abc + 3 * N;
+    T sa = 0, sap = 0, sb = 0, sbp = 0;
+    if (na > 0) q2d_list_sum<T, SLOPES>(da, abc, na, m == 1, x, sa, sap);
+    if (nb > 0) q2d_list_sum<T, SLOPES>(da + na, abc, nb, m == 1, x, sb, sbp);
+    P = o_fma(um, o_fma(cm, sa, sm * sb), P);
+    if (SLOPES) {
+      const T mm = (T)m, tx = (T)2 * x;
+      DR = o_fma(um1, o_fma(cm, o_fma(tx, sap, mm * sa), sm * o_fma(tx, sbp, mm * sb)), DR);
+      DT = o_fma(mm * um, o_fma(cm, sb, -sm * sa), DT);
+    }
+    um1 = um;
+    p = da + na + nb;
+  }
+}
+// r^2 = x^2 + y^2 unfused and u = rho / norm_radius by division, as the reference forms them: the departure's u > 1 cut is
+// a jump, and a point on the normalisation circle must fall on the reference's side of it
+template <typename T>
+OLB_HD T q2d_sag(T x, T y, const PrepSurface<T>& S, const T* pool) {
+  const T r2 = o_mul_nc(x, x) + o_mul_nc(y, y);
+  T zb = 0;                                              // _base_sag (geometry.py:117-131)
+  if (!(S.flags & PSF_RADIUS_INF)) {
+    T arg = (T)1 - S.kp1 * r2 * S.curv * S.curv;
+    zb = o_div(r2 * S.curv, (T)1 + o_sqrt(arg < 0 ? (T)0 : arg));
+  }
+  const T* blk = pool + S.coef_off;
+  const T u = o_div(o_sqrt(r2 + (T)1e-12), blk[Q2_NORM]);   // the sag's rho carries + 1e-12 (geometry.py:553)
+  if (u > (T)1) return zb;
+  const T usq = u * u;
+  // theta = atan2(y, x): rho + 1e-12 >= 1e-6, so the reference's x + 1e-12 guard never applies; at x = y = 0,
+  // atan2(+-0, x) is 0 or pi by the sign of x
+  T c1, s1 = 0;
+  const T rr = o_sqrt(r2);
+  if (rr > 0) { const T inv = o_rcp(rr); c1 = x * inv; s1 = y * inv; }
+  else c1 = copysign((T)1, x);
+  T S0 = 0, dS0, P, DR, DT, phi, dphi;
+  if (S.poly_rows > 0) forbes_q_sum(blk + Q2_HDR, S.poly_rows, usq, S0, dS0);
+  q2d_angular<T, false>(blk + Q2_HDR + S.poly_rows, S.n_coef, u, usq, c1, s1, P, DR, DT);
+  forbes_phi(r2, S, phi, dphi);
+  return zb + phi * o_fma(usq * ((T)1 - usq), S0, P);
+}
+template <typename T>
+OLB_HD void q2d_slopes(T x, T y, const PrepSurface<T>& S, const T* pool, T& fx, T& fy) {
+  const T* blk = pool + S.coef_off;
+  const T r2 = o_mul_nc(x, x) + o_mul_nc(y, y);
+  const T rho = o_sqrt(r2);                              // no + 1e-12 here (geometry.py:628-633)
+  if (rho < (T)1e-12) { fx = blk[Q2_VX]; fy = blk[Q2_VY]; return; }   // the vertex value (geometry.py:596-609)
+  const T inv_rho = o_rcp(rho);
+  const T c1 = x * inv_rho, s1 = y * inv_rho;
+  T db = 0;                                              // _base_sag_derivative (geometry.py:133-149)
+  if (!(S.flags & PSF_RADIUS_INF) && S.curv != 0) {
+    const T arg = (T)1 - S.kp1 * S.curv * S.curv * r2;
+    db = o_div(S.curv * rho, o_sqrt(arg > 0 ? arg : (T)1e-12));
+  }
+  T dsr = 0, dst = 0;
+  const T u = o_div(rho, blk[Q2_NORM]);
+  if (!(u > (T)1)) {
+    const T usq = u * u;
+    T S0 = 0, dS0 = 0, P, DR, DT, phi, dphi;
+    if (S.poly_rows > 0) forbes_q_sum(blk + Q2_HDR, S.poly_rows, usq, S0, dS0);
+    q2d_angular<T, true>(blk + Q2_HDR + S.poly_rows, S.n_coef, u, usq, c1, s1, P, DR, DT);
+    forbes_phi(r2, S, phi, dphi);
+    const T pre = usq - usq * usq;
+    const T dpref = ((T)2 * u - (T)4 * u * usq) * S.inv_norm;
+    const T dS0_drho = dS0 * (T)2 * u * S.inv_norm;
+    dsr = (dpref * S0 + pre * dS0_drho) * phi + pre * S0 * dphi + dphi * P + phi * DR * S.inv_norm;
+    dst = phi * DT;
+  }
+  const T g = db + dsr, h = dst * inv_rho;
+  fx = o_fma(c1, g, -s1 * h);
+  fy = o_fma(s1, g, c1 * h);
+}
+
 // FEAT: the Forbes code is compiled only into the general kernel (FEAT_EXTRA) -- inlined into the lean
 // Newton kernel it slows the even-asphere systems down (registers, I-cache); a table with
 // a Forbes surface is routed to the general kernel by prepare_table.
 template <typename T, uint32_t FEAT = 0xffffffffu>
 OLB_HD T newton_sag(T x, T y, const PrepSurface<T>& S, const T* pool, int& status) {
+  if constexpr ((FEAT & FEAT_Q2D) != 0) {                 // Q-2D: only in the two kernels of Q-2D tables
+    if (S.kind == OLB_GEOM_FORBES_Q2D) return q2d_sag(x, y, S, pool);
+  }
   if constexpr ((FEAT & FEAT_EXTRA) != 0) {
     if (S.kind == OLB_GEOM_FORBES_QBFS) return forbes_sag(x, y, S, pool);
   }
@@ -515,6 +625,9 @@ OLB_HD T newton_sag(T x, T y, const PrepSurface<T>& S, const T* pool, int& statu
 // reproducing the reference's eps-regularised chain rule).
 template <typename T, uint32_t FEAT = 0xffffffffu>
 OLB_HD void newton_slopes(T x, T y, const PrepSurface<T>& S, const T* pool, T& fx, T& fy) {
+  if constexpr ((FEAT & FEAT_Q2D) != 0) {
+    if (S.kind == OLB_GEOM_FORBES_Q2D) { q2d_slopes(x, y, S, pool, fx, fy); return; }
+  }
   if constexpr ((FEAT & FEAT_EXTRA) != 0) {
     if (S.kind == OLB_GEOM_FORBES_QBFS) { forbes_slopes(x, y, S, pool, fx, fy); return; }
   }

@@ -16,6 +16,7 @@
 
 #include <stdint.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <string>
@@ -39,7 +40,15 @@ enum : uint32_t {
   FEAT_GRID = 1u << 8,     // a grid-sag surface: the general kernel (polarized: + JONES) + PHASE + GRATING + this
   FEAT_POLYGON = 1u << 9,  // a polygon in an aperture program: the grid-sag superset + this
   FEAT_BSDF = 1u << 10,    // a BSDF scatter (OLB_SF_BSDF): the polygon superset + this (unpolarized only)
+  FEAT_Q2D = 1u << 11,     // a Forbes Q-2D surface: the general kernel (plain or polarized) + this, nothing else
 };
+
+// Prepared Forbes Q-2D block (PrepSurface::coef_off; n_coef = M, poly_rows = n0), elements of T:
+//   {vertex slope x, vertex slope y, norm_radius, 0}, the m = 0 list in the Q-bfs Clenshaw basis (n0), then per m = 1 .. M
+//   {na, nb, N = max(na, nb), 0}, N rows {A(n, m), B(n, m), C(n + 1, m)} of abc_q2d_clenshaw (qpoly.py:373-400), the
+//   cosine list in the Clenshaw basis (na), the sine list (nb).  The blocks follow each other without padding.
+enum { Q2_VX = 0, Q2_VY = 1, Q2_NORM = 2, Q2_HDR = 4, Q2_NA = 0, Q2_NB = 1, Q2_N = 2, Q2_MHDR = 4 };
+
 
 // Prepared BSDF block of a surface with OLB_SF_BSDF: BS_LEN elements of T right BEFORE its prepared media block (the
 // kernel finds it from PrepSurface::media_off alone; a BSDF table never runs the polarized kernels, whose coating
@@ -208,6 +217,90 @@ static inline void zernike_add_monomials(int n, int m, double coef, int deg, dou
   }
 }
 
+// Change of basis a_m -> b_m of the orthonormal polynomials the Q-bfs Clenshaw recurrence runs on
+// (G. W. Forbes, Opt. Express 18, 19700 (2010), eqs. A.14-A.16; geometries/forbes/qpoly.py:56-115):
+//   f_0 = 2, f_1 = sqrt(19)/2, g_0 = -1/2, h_{n-2} = -n(n-1) / (2 f_{n-2}),
+//   g_{n-1} = -(1 + g_{n-2} h_{n-2}) / f_{n-1}, f_n = sqrt(n(n+1) + 3 - g_{n-1}^2 - h_{n-2}^2)
+static inline void qbfs_change_basis(const double* a, int nc, std::vector<double>& b) {
+  std::vector<double> f(nc + 2), g(nc + 2), h(nc + 2);
+  b.assign(nc, 0.0);
+  for (int n = 0; n < nc; ++n) {
+    if (n == 0) f[0] = 2.0;
+    else if (n == 1) { g[0] = -0.5; f[1] = std::sqrt(19.0) / 2.0; }
+    else {
+      h[n - 2] = -(double)n * (n - 1) / (2.0 * f[n - 2]);
+      g[n - 1] = -(1.0 + g[n - 2] * h[n - 2]) / f[n - 1];
+      f[n] = std::sqrt((double)n * (n + 1) + 3.0 - g[n - 1] * g[n - 1] - h[n - 2] * h[n - 2]);
+    }
+  }
+  const int m = nc - 1;
+  if (m >= 0) b[m] = a[m] / f[m];
+  if (m >= 1) b[m - 1] = (a[m - 1] - g[m - 1] * b[m]) / f[m - 1];
+  for (int i = m - 2; i >= 0; --i) b[i] = (a[i] - g[i] * b[i + 1] - h[i] * b[i + 2]) / f[i];
+}
+
+// Recurrence constants of Forbes' Q-2D polynomials (G. W. Forbes, Opt. Express 20, 2483 (2012); the reference's
+// qpoly.py:26-40 and 289-400), in fp64 on the host.  Only the (n, m) the reference evaluates reach them: gamma with
+// n >= 1 and m >= 2.
+static inline double q2d_gamma(int n, int m) {
+  if (n == 1 && m == 2) return 3.0 / 8.0;
+  if (n == 1 && m > 2) {
+    const int mm1 = m - 1;
+    return ((double)(2 * mm1 + 1) / (double)(2 * (mm1 - 1))) * q2d_gamma(1, mm1);
+  }
+  const int nm1 = n - 1;
+  return ((double)((nm1 + 1) * (2 * m + 2 * nm1 - 1)) / (double)((m + nm1 - 2) * (2 * nm1 + 1))) * q2d_gamma(nm1, m);
+}
+static inline double q2d_dfact(int k) {   // k!! (odd k >= -1)
+  double f = 1;
+  for (int i = k; i > 1; i -= 2) f *= i;
+  return f;
+}
+static inline double q2d_g_raw(int n, int m) {
+  if (n == 0) return q2d_dfact(2 * m - 1) / (std::ldexp(1.0, m + 1) * fact(m - 1));
+  if (m == 1) {
+    const double t1 = -(double)((2 * n * n - 1) * (n * n - 1)) / (double)(8 * (4 * n * n - 1));
+    return t1 - (n == 1 ? 1.0 / 24.0 : 0.0);
+  }
+  const double num = (double)(2 * n * (m + n - 1) - m) * (double)((n + 1) * (2 * m + 2 * n - 1));
+  const double den = (double)((m + 2 * n - 2) * (m + 2 * n - 1)) * (double)((m + 2 * n) * (2 * n + 1));
+  return (-num / den) * q2d_gamma(n, m);
+}
+static inline double q2d_f_raw(int n, int m) {
+  if (n == 0 && m == 1) return 0.25;
+  if (n == 0) return (double)(m * m) * q2d_dfact(2 * m - 3) / (std::ldexp(1.0, m + 1) * fact(m - 1));
+  if (m == 1) {
+    const double t1 = (double)(4 * (n - 1) * (n - 1) * n * n + 1) / (double)(8 * (2 * n - 1) * (2 * n - 1));
+    return t1 + (n == 1 ? 11.0 / 32.0 : 0.0);
+  }
+  const int chi = m + n - 2;
+  const double num = (double)(2 * n * chi * (3 - 5 * m + 4 * n * chi)) + (double)(m * m * (3 - m + 4 * n * chi));
+  const double den = (double)((m + 2 * n - 3) * (m + 2 * n - 2)) * (double)((m + 2 * n - 1) * (2 * n - 1));
+  return (num / den) * q2d_gamma(n, m);
+}
+// f_q2d / g_q2d for n = 0 .. N-1 of one m (the recursion of qpoly.py:340-352 unrolled upwards)
+static inline void q2d_fg(int N, int m, std::vector<double>& f, std::vector<double>& g) {
+  f.assign(N, 0.0); g.assign(N, 0.0);
+  for (int n = 0; n < N; ++n) {
+    f[n] = n == 0 ? std::sqrt(q2d_f_raw(0, m)) : std::sqrt(q2d_f_raw(n, m) - g[n - 1] * g[n - 1]);
+    g[n] = q2d_g_raw(n, m) / f[n];
+  }
+}
+// abc_q2d_clenshaw(n, m): the reference's special cases (keyed (m, n)), else abc_q2d
+static inline void q2d_abc(int n, int m, double& A, double& B, double& C) {
+  if (m == 1 && n == 0) { A = 2; B = -1; C = 0; return; }
+  if (m == 1 && n == 1) { A = -4.0 / 3.0; B = -8.0 / 3.0; C = -11.0 / 3.0; return; }
+  if (m == 1 && n == 2) { A = 9.0 / 5.0; B = -24.0 / 5.0; C = 0; return; }
+  if (m == 2 && n == 0) { A = 3; B = -2; C = 0; return; }
+  if (m == 3 && n == 0) { A = 5; B = -4; C = 0; return; }
+  double d = (double)(4 * n * n - 1) * (double)(m + n - 2) * (double)(m + 2 * n - 3);
+  if (d == 0) d = 1e-99;
+  const double t1 = (double)((2 * n - 1) * (m + 2 * n - 2)), t2 = (double)(4 * n * (m + n - 2) + (m - 3) * (2 * m - 1));
+  A = (t1 * t2) / d;
+  B = (double)(-2 * (2 * n - 1) * (m + 2 * n - 3) * (m + 2 * n - 2) * (m + 2 * n - 1)) / d;
+  C = (double)(n * (2 * n - 3) * (m + 2 * n - 1) * (2 * m + 2 * n - 3)) / d;
+}
+
 enum : uint32_t { HINT_POLY_NEWTON = 1u };   // a polynomial-family / biconic / toroidal Newton surface is present
 struct PrepResult {
   std::vector<unsigned char> blob_f64, blob_f32;
@@ -347,7 +440,7 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
   std::vector<std::vector<double>> pools(tab.n_surfaces);
   uint32_t features = 0;
   int prev = -1;  // previous surface with a frame (non-NOOP)
-  int64_t grid_elements = 0, polygon_vertices = 0;
+  int64_t grid_elements = 0, polygon_vertices = 0, q2d_elements = 0;
   std::vector<std::vector<PolygonSource>> polygons(tab.n_surfaces);
   auto in_pool = [&](int off, int len) { return off >= 0 && len >= 0 && (int64_t)off + len <= tab.pool_len; };
 
@@ -360,7 +453,7 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     o.flags = in.flags & 0xffu;
     o.max_iter = in.max_iter;
     o.coating = in.coating;
-    if (in.kind < OLB_GEOM_NOOP || in.kind > OLB_GEOM_GRID_SAG) { res.error = "unknown geometry kind"; return res; }
+    if (in.kind < OLB_GEOM_NOOP || in.kind > OLB_GEOM_FORBES_Q2D) { res.error = "unknown geometry kind"; return res; }
 
     // ---- pose --------------------------------------------------------------
     if (in.kind != OLB_GEOM_NOOP) {
@@ -515,34 +608,90 @@ static inline PrepResult prepare_table(const OlbTable& tab) {
     } else if (in.kind == OLB_GEOM_FORBES_QBFS) {
       if (in.n_coef < 0 || in.n_coef > 64 || !in_pool(in.coef_off, in.n_coef)) { res.error = "bad Forbes coefficient block"; return res; }
       if (!(in.norm_radius > 0)) { res.error = "Forbes norm_radius must be positive"; return res; }
-      // Change of basis a_m -> b_m of the orthonormal polynomials the Clenshaw recurrence runs on
-      // (G. W. Forbes, Opt. Express 18, 19700 (2010), eqs. A.14-A.16; geometries/forbes/qpoly.py:56-115):
-      //   f_0 = 2, f_1 = sqrt(19)/2, g_0 = -1/2, h_{n-2} = -n(n-1) / (2 f_{n-2}),
-      //   g_{n-1} = -(1 + g_{n-2} h_{n-2}) / f_{n-1}, f_n = sqrt(n(n+1) + 3 - g_{n-1}^2 - h_{n-2}^2)
       const int nc = in.n_coef;
-      std::vector<double> f(nc + 2), g(nc + 2), h(nc + 2), b(nc, 0.0);
-      for (int n = 0; n < nc; ++n) {
-        if (n == 0) f[0] = 2.0;
-        else if (n == 1) { g[0] = -0.5; f[1] = std::sqrt(19.0) / 2.0; }
-        else {
-          h[n - 2] = -(double)n * (n - 1) / (2.0 * f[n - 2]);
-          g[n - 1] = -(1.0 + g[n - 2] * h[n - 2]) / f[n - 1];
-          f[n] = std::sqrt((double)n * (n + 1) + 3.0 - g[n - 1] * g[n - 1] - h[n - 2] * h[n - 2]);
-        }
-      }
       const double* a = tab.pool + in.coef_off;
-      const int m = nc - 1;
+      std::vector<double> b;
+      qbfs_change_basis(a, nc, b);
       bool all_zero = true;
       for (int i = 0; i < nc; ++i) all_zero = all_zero && a[i] == 0.0;
-      if (m >= 0) b[m] = a[m] / f[m];
-      if (m >= 1) b[m - 1] = (a[m - 1] - g[m - 1] * b[m]) / f[m - 1];
-      for (int i = m - 2; i >= 0; --i) b[i] = (a[i] - g[i] * b[i + 1] - h[i] * b[i + 2]) / f[i];
       o.n_coef = all_zero ? 0 : nc;    // no / all-zero terms: the reference's slope takes the base-conic branch
       o.coef_off = (int)pool.size();
       for (int i = 0; i < nc; ++i) pool.push_back(b[i]);
       while (pool.size() % 4) pool.push_back(0);
       o.inv_norm = 1.0 / in.norm_radius;
       features |= FEAT_EXTRA;          // the Forbes code lives in the general kernel only (olb_math.cuh::newton_sag)
+    } else if (in.kind == OLB_GEOM_FORBES_Q2D) {
+      // cm0[n0], {na_m, nb_m} x M, then the lists (include/olb.h "Forbes Q-2D")
+      const int n0 = in.aux0, M = in.n_coef;
+      if (M < 0 || M > OLB_Q2D_MAX_M) { res.error = "Forbes Q-2D: M out of range (max " + std::to_string(OLB_Q2D_MAX_M) + ")"; return res; }
+      if (n0 < 0 || n0 > OLB_Q2D_MAX_TERMS || !in_pool(in.coef_off, n0 + 2 * M)) { res.error = "bad Forbes Q-2D block"; return res; }
+      if (!(in.norm_radius > 0) || !std::isfinite(in.norm_radius)) { res.error = "Forbes Q-2D norm_radius must be positive and finite"; return res; }
+      const double* blk = tab.pool + in.coef_off;
+      std::vector<int> na(M), nb(M);
+      int len = n0 + 2 * M;
+      int64_t elems = Q2_HDR + n0;
+      for (int m = 0; m < M; ++m) {
+        const double da = blk[n0 + 2 * m], db = blk[n0 + 2 * m + 1];
+        if (!(da >= 0 && da <= OLB_Q2D_MAX_TERMS && da == std::floor(da)) || !(db >= 0 && db <= OLB_Q2D_MAX_TERMS && db == std::floor(db))) {
+          res.error = "Forbes Q-2D: list lengths must be integers in [0, " + std::to_string(OLB_Q2D_MAX_TERMS) + "]"; return res;
+        }
+        na[m] = (int)da; nb[m] = (int)db;
+        len += na[m] + nb[m];
+        elems += Q2_MHDR + 3 * std::max(na[m], nb[m]) + na[m] + nb[m];
+      }
+      if (!in_pool(in.coef_off, len)) { res.error = "Forbes Q-2D block outside pool"; return res; }
+      for (int k = 0; k < len; ++k)
+        if (!std::isfinite(blk[k])) { res.error = "Forbes Q-2D: non-finite coefficient"; return res; }
+      q2d_elements += elems;
+      if (q2d_elements > OLB_MAX_Q2D_ELEMENTS) {
+        res.error = "Forbes Q-2D: the surfaces of this table exceed " + std::to_string(OLB_MAX_Q2D_ELEMENTS) +
+                    " prepared elements (they are staged in shared memory)";
+        return res;
+      }
+      while (pool.size() % 4) pool.push_back(0);
+      o.coef_off = (int)pool.size();
+      o.n_coef = M; o.poly_rows = n0;
+      o.inv_norm = 1.0 / in.norm_radius;
+      pool.insert(pool.end(), Q2_HDR, 0.0);
+      pool[o.coef_off + Q2_NORM] = in.norm_radius;
+      std::vector<double> b;
+      qbfs_change_basis(blk, n0, b);                 // m = 0: compute_z_zprime_qbfs (qpoly.py:265-283)
+      pool.insert(pool.end(), b.begin(), b.end());
+      const double* lists = blk + n0 + 2 * M;
+      for (int m = 1; m <= M; ++m) {
+        const int N = std::max(na[m - 1], nb[m - 1]);
+        std::vector<double> f, g;
+        q2d_fg(N, m, f, g);
+        pool.push_back(na[m - 1]); pool.push_back(nb[m - 1]); pool.push_back(N); pool.push_back(0);
+        const size_t abc = pool.size();
+        for (int n = 0; n < N; ++n) {
+          double A, B, C, A1, B1, C1;
+          q2d_abc(n, m, A, B, C);
+          q2d_abc(n + 1, m, A1, B1, C1);
+          pool.push_back(A); pool.push_back(B); pool.push_back(C1);
+        }
+        for (int side = 0; side < 2; ++side) {
+          const int nl = side == 0 ? na[m - 1] : nb[m - 1];
+          const double* c = lists;
+          lists += nl;
+          // change_basis_q2d_to_pnm (qpoly.py:355-370)
+          std::vector<double> d(nl);
+          for (int n = nl - 1; n >= 0; --n) d[n] = n == nl - 1 ? c[n] / f[n] : (c[n] - g[n] * d[n + 1]) / f[n];
+          if (m == 1 && nl > 0) {
+            // vertex slope (geometry.py:596-609): the m = 1 sum at usq = 0, divided by norm_radius
+            double a1 = 0, a2 = 0, a0 = 0, a3 = 0;
+            for (int n = nl - 1; n >= 0; --n) {
+              a0 = d[n] + pool[abc + 3 * n] * a1 - pool[abc + 3 * n + 2] * a2;
+              if (n == 3) a3 = a0;
+              a2 = a1; a1 = a0;
+            }
+            pool[o.coef_off + (side == 0 ? Q2_VX : Q2_VY)] = (0.5 * a0 - (nl > 3 ? 2.0 / 5.0 * a3 : 0.0)) / in.norm_radius;
+          }
+          pool.insert(pool.end(), d.begin(), d.end());
+        }
+      }
+      while (pool.size() % 4) pool.push_back(0);
+      features |= FEAT_EXTRA | FEAT_Q2D;
     } else if (in.kind == OLB_GEOM_ZERNIKE) {
       if (!in_pool(in.coef_off, 4 * in.n_coef)) { res.error = "Zernike block outside pool"; return res; }
       if (!(in.norm_radius > 0)) { res.error = "Zernike norm_radius must be positive"; return res; }
@@ -858,6 +1007,10 @@ static BatchPrep prepare_batch(const OlbTable& tmpl, const double* params, int n
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].kind == OLB_GEOM_GRID_SAG) {
       out.error = "batched tables with grid-sag surfaces are not built"; out.unsupported = true; return out;
+    }
+  for (int s = 0; s < S && tmpl.surfaces; ++s)
+    if (tmpl.surfaces[s].kind == OLB_GEOM_FORBES_Q2D) {
+      out.error = "batched tables with Forbes Q-2D surfaces are not built"; out.unsupported = true; return out;
     }
   for (int s = 0; s < S && tmpl.surfaces; ++s)
     if (tmpl.surfaces[s].coating >= OLB_COAT_THIN_FILM && tmpl.surfaces[s].coating <= OLB_COAT_RETARDER) {

@@ -865,6 +865,10 @@ static int launch_instance(const TraceArgs& a, cudaStream_t stream) {
 }
 
 constexpr uint32_t FEAT_GENERAL = FEAT_ROT | FEAT_NEWTON | FEAT_EXTRA | FEAT_FREEFORM;
+// What a Q-2D table may not hold: its two kernel variants carry none of these code paths
+constexpr uint32_t FEAT_Q2D_EXCLUDED = FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON | FEAT_BSDF | FEAT_JONES;
+static const char* const Q2D_EXCLUDED_MSG = "a Forbes Q-2D surface in a table with a phase profile, ruled grating, grid "
+                                            "sag, polygon aperture, BSDF or thin-film / polarizer / retarder coating is not built";
 
 template <typename T, int RPT>
 static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t stream) {
@@ -874,6 +878,10 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
       // cache (no_instruction was the second largest stall of the Zernike + Fresnel configuration)
       const uint32_t g = features & ~FEAT_POL;
       if (g & FEAT_BSDF) return fail(OLB_ERR_UNSUPPORTED, "polarized trace of a table with a BSDF surface is not built");
+      if (g & FEAT_Q2D) {      // Forbes Q-2D surfaces: the general polarized kernel + the Q-2D sag, and nothing else
+        if (g & FEAT_Q2D_EXCLUDED) return fail(OLB_ERR_UNSUPPORTED, Q2D_EXCLUDED_MSG);
+        return launch_instance<T, 1, FEAT_GENERAL | FEAT_POL | FEAT_Q2D>(a, stream);
+      }
       if (g & FEAT_POLYGON)      // polygon apertures: the grid-sag superset + the polygon scan, so a polygon works on any surface
         return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_POL | FEAT_JONES | FEAT_GRID | FEAT_POLYGON>(a, stream);
       if (g & FEAT_GRID)         // grid-sag surfaces: the superset below, so every coating and DOE works on a grid
@@ -895,6 +903,10 @@ static int launch_feat(const TraceArgs& a, uint32_t features, cudaStream_t strea
   // tables with a ruled grating (phase surfaces allowed beside it) add the grating interaction to that, and tables with
   // a grid-sag surface the grid loop to both; tables with a polygon aperture the polygon scan to all three; tables with
   // a BSDF surface the scatter to all four, so a BSDF works on every geometry, interaction and aperture
+  if (features & FEAT_Q2D) {    // Forbes Q-2D surfaces: the general kernel + the Q-2D sag, one ray per thread
+    if (features & FEAT_Q2D_EXCLUDED) return fail(OLB_ERR_UNSUPPORTED, Q2D_EXCLUDED_MSG);
+    return launch_instance<T, 1, FEAT_GENERAL | FEAT_Q2D>(a, stream);
+  }
   if (features & FEAT_BSDF)
     return launch_instance<T, 1, FEAT_GENERAL | FEAT_PHASE | FEAT_GRATING | FEAT_GRID | FEAT_POLYGON | FEAT_BSDF>(a, stream);
   if (features & FEAT_POLYGON)
@@ -1166,7 +1178,7 @@ static int aim_impl(const OlbDeviceTable* wh, const OlbAimCall& c, cudaStream_t 
   if (c.max_iter < 0) return fail(OLB_ERR_INVALID_ARG, "max_iter < 0");
   if (!c.status) return fail(OLB_ERR_INVALID_ARG, "status is NULL");
   const int variant = aim_variant(wh->features);
-  if (variant < 0) return fail(OLB_ERR_UNSUPPORTED, "ray aiming through a BSDF surface or a polarizing coating is not built");
+  if (variant < 0) return fail(OLB_ERR_UNSUPPORTED, "ray aiming through a BSDF surface, a polarizing coating or a Forbes Q-2D surface is not built");
   if (c.n_rays == 0) return OLB_OK;
   if (!c.rays) return fail(OLB_ERR_INVALID_ARG, "rays is NULL");
   const OlbRays& r = *c.rays;

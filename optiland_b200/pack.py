@@ -105,6 +105,9 @@ class _Prefetch:
             if _cls(g) == "GridSagGeometry":       # the node coordinates and sag values (pack_grid_sag)
                 for k in ("x_grid", "y_grid", "sag_grid"):
                     self._add_array(getattr(g, k, None))
+            if _cls(g) == "ForbesQ2dGeometry":     # the grouped coefficient lists (pack_forbes_q2d)
+                for k in ("cm0_coeffs", "ams_coeffs", "bms_coeffs"):
+                    self._add(getattr(g, k, None))
             for k in ("coefficients", "coeffs_poly_y"):
                 c = getattr(g, k, None)
                 if isinstance(c, (list, tuple)):
@@ -293,6 +296,7 @@ _GEOM_KINDS = {
     "ToroidalGeometry": T.GEOM_TOROIDAL,
     "ForbesQNormalSlopeGeometry": T.GEOM_FORBES_QBFS,
     "ForbesQbfsGeometry": T.GEOM_FORBES_QBFS,       # deprecated alias class (forbes/geometry.py:733-759)
+    "ForbesQ2dGeometry": T.GEOM_FORBES_Q2D,
 }
 
 
@@ -344,6 +348,46 @@ def pack_grid_sag(spec: T.SurfaceSpec, g) -> None:
     spec.grid_x, spec.grid_y, spec.grid_sag = x.copy(), y.copy(), z.copy()
     spec.tol = float(g.tol)
     spec.max_iter = int(g.max_iter)
+
+
+def pack_forbes_q2d(spec: T.SurfaceSpec, g) -> None:
+    """``ForbesQ2dGeometry`` (optiland/geometries/forbes/geometry.py:445-731) -> ``spec``: the coefficient lists in the
+    reference's own grouping (``cm0_coeffs``, ``ams_coeffs``, ``bms_coeffs``, built by ``_prepare_coeffs`` -- what its sag
+    and normal read) and the live ``norm_radius``.  Lists over the caps (``T.Q2D_MAX_M``, ``T.Q2D_MAX_TERMS``) and
+    non-finite coefficients decline, each with a reason."""
+    ams, bms = list(g.ams_coeffs or []), list(g.bms_coeffs or [])
+    if len(ams) != len(bms):
+        raise UnsupportedSurface(f"Forbes Q-2D with {len(ams)} cosine and {len(bms)} sine lists")
+    if len(ams) > T.Q2D_MAX_M:
+        raise UnsupportedSurface(f"Forbes Q-2D with azimuthal order {len(ams)} (max {T.Q2D_MAX_M})")
+    lists = [np.array([_f(c) for c in v], dtype=np.float64) for v in [list(g.cm0_coeffs or []), *ams, *bms]]
+    if any(len(v) > T.Q2D_MAX_TERMS for v in lists):
+        raise UnsupportedSurface(f"Forbes Q-2D with radial order above {T.Q2D_MAX_TERMS - 1}")
+    if not all(np.all(np.isfinite(v)) for v in lists):
+        raise UnsupportedSurface("Forbes Q-2D with non-finite coefficients")
+    norm = _f(g.norm_radius)
+    if not (np.isfinite(norm) and norm > 0):
+        raise UnsupportedSurface(f"Forbes Q-2D with norm_radius {norm}")
+    M = len(ams)
+    spec.q2d_cm0, spec.q2d_ams, spec.q2d_bms = lists[0], lists[1:1 + M], lists[1 + M:]
+    spec.norm_radius = norm
+
+
+# what the two kernel variants of Q-2D tables do not carry (olb_trace.cu: FEAT_Q2D_EXCLUDED)
+def _q2d_excluded(spec: T.SurfaceSpec) -> str | None:
+    if spec.interaction == T.INTERACT_GRATING:
+        return "ruled grating"
+    if spec.interaction != T.INTERACT_REFRACT:
+        return "phase profile"
+    if spec.kind == T.GEOM_GRID_SAG:
+        return "grid sag"
+    if spec.bsdf != T.BSDF_NONE:
+        return "BSDF"
+    if spec.coating in T.JONES_COATINGS:
+        return "thin-film, polarizer or retarder coating"
+    if spec.aperture is not None and T.polygon_vertices(spec.aperture):
+        return "polygon aperture"
+    return None
 
 
 _GRATING_KINDS = {"PlaneGrating": T.GEOM_PLANE, "StandardGratingGeometry": T.GEOM_STANDARD}
@@ -542,6 +586,8 @@ def pack_surface(surface, wavelengths, position: int = 0) -> T.SurfaceSpec:
             raise UnsupportedSurface("Forbes radial term with a negative order")
         spec.coefficients = np.array([terms.get(n, 0.0) for n in range(max(terms) + 1)] if terms else [], dtype=np.float64)
         spec.norm_radius = _f(g.norm_radius)
+    elif kind == T.GEOM_FORBES_Q2D:
+        pack_forbes_q2d(spec, g)
     elif kind == T.GEOM_ZERNIKE:
         z = g.zernike
         coeffs = [_f(c) for c in z.coeffs]
@@ -601,6 +647,16 @@ def pack_surface_group(surface_group, wavelengths) -> T.SurfaceTable:
         if nv > T.MAX_POLYGON_VERTICES:
             raise UnsupportedSurface(f"polygon apertures with {nv} vertices in all: more than {T.MAX_POLYGON_VERTICES} "
                                      "prepared in shared memory")
+        q2d = [s for s in specs if s.kind == T.GEOM_FORBES_Q2D]
+        if q2d:
+            ne = sum(T.q2d_elements(s.q2d_cm0, s.q2d_ams, s.q2d_bms) for s in q2d)
+            if ne > T.MAX_Q2D_ELEMENTS:
+                raise UnsupportedSurface(f"Forbes Q-2D surfaces with {ne} prepared elements in all: more than "
+                                         f"{T.MAX_Q2D_ELEMENTS} in shared memory")
+            for s in specs:
+                what = _q2d_excluded(s)
+                if what is not None:
+                    raise UnsupportedSurface(f"Forbes Q-2D surface beside a {what}")
         return T.SurfaceTable(specs, wavelengths)
 
 

@@ -797,6 +797,9 @@ def _wants_grad(backend, surfaces, rays=None) -> bool:
         rt = getattr(g, "radial_terms", None)        # Forbes Q^bfs: {order: tensor}
         if isinstance(rt, dict):
             vals += list(rt.values())
+        ff = getattr(g, "freeform_coeffs", None)     # Forbes Q-2D: {(kind, m, n): tensor} (pack.pack_forbes_q2d)
+        if isinstance(ff, dict):
+            vals += list(ff.values()) + [getattr(g, "norm_radius", None)]
         coefs = getattr(g, "coefficients", None)     # (Zernike: the property returns geometry.zernike.coeffs)
         if coefs is not None:
             vals += [coefs] if hasattr(coefs, "requires_grad") else list(np.ravel(np.asarray(coefs, dtype=object)))
@@ -1026,6 +1029,9 @@ def _device_aim_solver(backend, aimer, probe, wavelengths):
     table = checked[0]
     if any(s.bsdf != T.BSDF_NONE for s in table.surfaces):
         _decline("robust ray aiming: BSDF surface before the stop")
+        return None
+    if any(s.kind == T.GEOM_FORBES_Q2D for s in table.surfaces):
+        _decline("robust ray aiming: Forbes Q-2D surface before the stop")
         return None
     if table.surfaces[-1].kind == T.GEOM_NOOP:
         return None                     # the stop is the object surface: it has no local frame in the kernel

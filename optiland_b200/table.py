@@ -39,6 +39,20 @@ MAX_GRID_ELEMENTS = 8192
 def grid_elements(nx: int, ny: int) -> int:
     return nx + ny + nx * ny
 
+
+GEOM_FORBES_Q2D = 12
+# Forbes Q-2D caps (include/olb.h): the highest azimuthal order m, the longest coefficient list (radial orders 0 .. 15),
+# and the prepared elements of one table, staged in shared memory with the rest of it (olb_prep.h)
+Q2D_MAX_M = 16
+Q2D_MAX_TERMS = 16
+MAX_Q2D_ELEMENTS = 4096
+
+
+def q2d_elements(cm0, ams, bms) -> int:
+    """Prepared elements of one Q-2D surface (olb_prep.h): a 4-element header, the m = 0 list, and per m a 4-element
+    header, the recurrence constants (3 per radial order of the longer list) and both lists."""
+    return 4 + len(cm0) + sum(4 + 3 * max(len(a), len(b)) + len(a) + len(b) for a, b in zip(ams, bms))
+
 SF_REFLECT = 1 << 0
 SF_ROTATED = 1 << 1
 SF_APERTURE = 1 << 2
@@ -104,7 +118,7 @@ MAX_SURFACES = 64
 MAX_WAVELENGTHS = 16
 
 NEWTON_KINDS = (GEOM_EVEN_ASPHERE, GEOM_ZERNIKE, GEOM_ODD_ASPHERE, GEOM_POLYNOMIAL, GEOM_CHEBYSHEV, GEOM_BICONIC,
-                GEOM_TOROIDAL, GEOM_FORBES_QBFS)
+                GEOM_TOROIDAL, GEOM_FORBES_QBFS, GEOM_FORBES_Q2D)
 
 # numpy mirror of `struct OlbSurface` (192 bytes)
 OLB_SURFACE_DTYPE = np.dtype(
@@ -184,6 +198,12 @@ class SurfaceSpec:
     bsdf: int = BSDF_NONE
     bsdf_sigma: float = 0.0
     bsdf_seed: int = 0
+    # Forbes Q-2D (GEOM_FORBES_Q2D, include/olb.h): the reference's grouping of the coefficients -- the m = 0 list and,
+    # for m = 1 .. M, the cosine and the sine lists (ForbesQ2dGeometry.cm0_coeffs / ams_coeffs / bms_coeffs), each
+    # indexed by the radial order n; norm_radius holds the normalisation radius
+    q2d_cm0: np.ndarray = field(default_factory=lambda: np.zeros(0))
+    q2d_ams: list = field(default_factory=list)
+    q2d_bms: list = field(default_factory=list)
 
     def __post_init__(self):
         self.t = np.asarray(self.t, dtype=np.float64).reshape(3)
@@ -211,6 +231,15 @@ class SurfaceSpec:
         self.grid_x = np.asarray(self.grid_x, dtype=np.float64).ravel()
         self.grid_y = np.asarray(self.grid_y, dtype=np.float64).ravel()
         self.grid_sag = np.atleast_2d(np.asarray(self.grid_sag, dtype=np.float64))
+        self.q2d_cm0 = np.asarray(self.q2d_cm0, dtype=np.float64).ravel()
+        self.q2d_ams = [np.asarray(a, dtype=np.float64).ravel() for a in self.q2d_ams]
+        self.q2d_bms = [np.asarray(b, dtype=np.float64).ravel() for b in self.q2d_bms]
+
+    def q2d_block(self) -> np.ndarray:
+        """The pool block of a Q-2D surface (include/olb.h): cm0, {na_m, nb_m} per m, then the lists a_1, b_1, a_2, ..."""
+        lens = [float(len(v)) for a, b in zip(self.q2d_ams, self.q2d_bms) for v in (a, b)]
+        lists = [v for a, b in zip(self.q2d_ams, self.q2d_bms) for v in (a, b)]
+        return np.concatenate([self.q2d_cm0, np.asarray(lens, dtype=np.float64), *lists])
 
     def coating_block(self) -> np.ndarray:
         """The pool block of a thin-film / polarizer / retarder coating (include/olb.h), empty for other coatings."""
@@ -370,6 +399,17 @@ class SurfaceTable:
                         raise ValueError(f"grid sag: {name} must be finite and strictly increasing")
                 if not np.all(np.isfinite(s.grid_sag)):
                     raise ValueError("grid sag: non-finite sag value")
+            if s.kind == GEOM_FORBES_Q2D:
+                if len(s.q2d_ams) != len(s.q2d_bms) or len(s.q2d_ams) > Q2D_MAX_M:
+                    raise ValueError(f"Forbes Q-2D: {len(s.q2d_ams)} cosine and {len(s.q2d_bms)} sine lists (equal, at most "
+                                     f"{Q2D_MAX_M})")
+                lists = [s.q2d_cm0, *s.q2d_ams, *s.q2d_bms]
+                if any(len(v) > Q2D_MAX_TERMS for v in lists):
+                    raise ValueError(f"Forbes Q-2D: a coefficient list longer than {Q2D_MAX_TERMS}")
+                if not all(np.all(np.isfinite(v)) for v in lists):
+                    raise ValueError("Forbes Q-2D: non-finite coefficient")
+                if not (np.isfinite(s.norm_radius) and s.norm_radius > 0):
+                    raise ValueError(f"Forbes Q-2D: norm_radius {s.norm_radius} must be positive and finite")
             if s.interaction == INTERACT_GRATING:
                 if s.kind not in (GEOM_PLANE, GEOM_STANDARD) or (s.kind == GEOM_STANDARD and not np.isfinite(s.radius)):
                     raise ValueError("grating: only on a plane or a conic with a finite radius")
@@ -396,6 +436,10 @@ class SurfaceTable:
         if grid > MAX_GRID_ELEMENTS:
             raise ValueError(f"grid-sag surfaces of this table need {grid} prepared elements in shared memory "
                              f"(more than {MAX_GRID_ELEMENTS})")
+        q2d = sum(q2d_elements(s.q2d_cm0, s.q2d_ams, s.q2d_bms) for s in self.surfaces if s.kind == GEOM_FORBES_Q2D)
+        if q2d > MAX_Q2D_ELEMENTS:
+            raise ValueError(f"Forbes Q-2D surfaces of this table need {q2d} prepared elements in shared memory "
+                             f"(more than {MAX_Q2D_ELEMENTS})")
 
     @property
     def num_surfaces(self) -> int:
@@ -445,6 +489,11 @@ class SurfaceTable:
                 coef = np.concatenate([s.grid_x, s.grid_y, s.grid_sag.ravel()])
                 ints["n_coef"][j] = len(s.grid_y)
                 ints["aux0"][j] = len(s.grid_x)
+            elif s.kind == GEOM_FORBES_Q2D:
+                # cm0[n0], {na_m, nb_m} x M, the lists (include/olb.h): aux0 = n0, n_coef = M
+                coef = s.q2d_block()
+                ints["n_coef"][j] = len(s.q2d_ams)
+                ints["aux0"][j] = len(s.q2d_cm0)
             else:
                 ints["n_coef"][j] = coef.size
             if extra_head is not None:
@@ -546,9 +595,19 @@ class SurfaceTable:
                 grid = dict(grid_x=g[:nx].copy(), grid_y=g[nx:nx + n_coef].copy(),
                             grid_sag=g[nx + n_coef:].reshape(n_coef, nx).copy())
                 coef = np.zeros(0)
+            elif kind == GEOM_FORBES_Q2D:
+                n0 = int(r["aux0"])
+                lens = pool[off + n0: off + n0 + 2 * n_coef].astype(int)
+                p = off + n0 + 2 * n_coef
+                lists = []
+                for ln in lens:
+                    lists.append(pool[p: p + ln].copy())
+                    p += ln
+                grid = dict(q2d_cm0=pool[off: off + n0].copy(), q2d_ams=lists[0::2], q2d_bms=lists[1::2])
+                coef = np.zeros(0)
             else:
                 coef = pool[off: off + n_coef].copy()
-            if kind != GEOM_GRID_SAG:
+            if kind not in (GEOM_GRID_SAG, GEOM_FORBES_Q2D):
                 grid = {}
             flags = int(r["flags"])
             aper = None
